@@ -2,7 +2,7 @@
 """Headline benchmark: frames/sec through the four trackers (BASELINE.json metric) on synthetic frames.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference|eager] [--config all4|players|pose|court|ball]
-                  [--batch B] [--res 1080p|4k|720p] [--strong [--frames N]]
+                  [--batch B] [--res 1080p|4k|720p] [--strong [--frames N]] [--dump-outputs DIR]
 
 One *step* = one batch of `--batch` frames through the hot path of the selected trackers (default all four:
 PlayerTracker YOLOv8n-detect, PlayerKeypointsTracker YOLOv8n-pose 13x3 @1280, KeypointsTracker YOLOv8n-pose 12x3 @640,
@@ -13,6 +13,9 @@ NCCL only broadcasts the weights at init and gathers detection counts at the end
 --strong: a FIXED job of --frames frames goes through `TrackingRunner.run()` (the reference's entry point) sharded over the
 ranks by contiguous ranges, with the result all_gather and the rank-0 host stages (polygon filter, ByteTrack, result
 objects) INSIDE the timed region ("scaling": "strong").
+
+--dump-outputs DIR: rank 0 writes the last timed batch's tracker results as DIR/<tracker>.npy (float64, fixed order);
+inputs and weights are seeded, so two builds can be compared output for output.
 
 Printed JSON (rank 0, one line): value (device-resident frames), e2e (pinned host frames through the tracker API, H2D
 and result D2H inside the timed region), roofline (dominant kernel, event-timed live), cpu_baseline (the CPU oracle on
@@ -48,11 +51,12 @@ def _peaks():
         d = json.loads(p.read_text())
         return dict(tflops_burst=d.get("bf16_tflops"), tflops_sustained=d.get("bf16_tflops_sustained"),
                     hbm_gbs=d.get("hbm_gbs"), source="measured")
-    return dict(tflops_burst=1590.0, tflops_sustained=1400.0, hbm_gbs=6650.0, source="fallback")
+    # H100 SXM data sheet (dense fp16 tensor core, HBM3), not measured
+    return dict(tflops_burst=989.0, tflops_sustained=989.0, hbm_gbs=3350.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -206,7 +210,7 @@ def run_reference_arm(args, rank, world):
 
 def run_eager_arm(args, rank, world):
     """`--impl eager`: the oracle networks (what ultralytics / the reference's TrackNet run) in PyTorch eager mode on
-    one B200 with cuDNN TF32 convolutions -- the reference's own GPU numerics, and the library baseline the hand-written
+    one GPU with cuDNN TF32 convolutions -- the reference's own GPU numerics, and the library baseline the hand-written
     conv kernels are measured against.  Timed per step: network forward (+ torchvision NMS for the YOLO heads) of every
     selected tracker on a resident, already pre-processed batch (the reference pre-processes on the CPU: cv2 / PIL)."""
     if rank != 0:
@@ -407,6 +411,48 @@ def run_strong(args, rank, world, local, dev):
         }), file=JSON_OUT, flush=True)
 
 
+def _numbers(obj, acc, seen):
+    """Every number reachable from a tracker result (arrays, scalars, lists, dicts, attributes in name order)."""
+    if obj is None or isinstance(obj, (str, bytes)):
+        return
+    if isinstance(obj, (bool, int, float, np.number)):
+        acc.append(float(obj))
+    elif isinstance(obj, torch.Tensor):
+        acc.extend(obj.detach().double().cpu().reshape(-1).tolist())
+    elif isinstance(obj, np.ndarray):
+        if obj.dtype.kind in "biuf":
+            acc.extend(obj.astype(np.float64).reshape(-1).tolist())
+        else:
+            for v in obj.reshape(-1):
+                _numbers(v, acc, seen)
+    elif id(obj) in seen:
+        return
+    else:
+        seen.add(id(obj))
+        if isinstance(obj, dict):
+            for k in sorted(obj, key=str):
+                _numbers(obj[k], acc, seen)
+        elif isinstance(obj, (list, tuple)):
+            for v in obj:
+                _numbers(v, acc, seen)
+        elif hasattr(obj, "__dict__"):
+            for k in sorted(vars(obj)):
+                _numbers(vars(obj)[k], acc, seen)
+
+
+def dump_outputs(out, d: Path):
+    """One float64 .npy per tracker of the last timed batch's results (64 MB cap: a seeded sample beyond it)."""
+    d.mkdir(parents=True, exist_ok=True)
+    for name, res in out.items():
+        acc = []
+        _numbers(res, acc, set())
+        a = np.asarray(acc, dtype=np.float64)
+        cap = (64 << 20) // 8 // max(1, len(out))
+        if a.size > cap:
+            a = a[np.sort(np.random.default_rng(0).choice(a.size, cap, replace=False))]
+        np.save(d / f"{name}.npy", a)
+
+
 def main():
     sys.stdout = sys.stderr
     ap = argparse.ArgumentParser()
@@ -421,6 +467,7 @@ def main():
     ap.add_argument("--frames", type=int, default=4096, help="--strong: frames of the fixed job")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--profile-host", action="store_true", help="cProfile the timed region's host side (stderr)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's tracker results as DIR/<name>.npy")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -466,7 +513,7 @@ def main():
     ball = trackers.get("ball")
 
     # frames: NBUF distinct batches resident in HBM (+ pinned host copies for the e2e leg); each batch (B*H*W*3 bytes
-    # = 199 MB at 1080p/32) alone exceeds the 126 MB L2 and activations are GBs, so no L2 flush is needed.
+    # = 199 MB at 1080p/32) alone exceeds the 50 MB L2 and activations are GBs, so no L2 flush is needed.
     NBUF = 3
     dev_batches = [synth.make_frames(B, H, W, start=rank * 100000 + i * B, device=dev) for i in range(NBUF)]
     host_batches = [b.cpu().pin_memory() for b in dev_batches]
@@ -479,10 +526,13 @@ def main():
     if ball is not None:
         ball._pipe.push_frames(dev_batches[0][:7])  # prime the 8-frame window so every step yields B windows
 
+    last = {}
+
     def run_steps(batches, steps):
         nd = 0
         for out in fused.run(batches[i % NBUF] for i in range(steps)):
             nd += sum(len(p) for k in ("players", "pose") if k in out for p in out[k])
+            last["out"] = out
         return nd
 
     import gc
@@ -525,6 +575,8 @@ def main():
         pr = cProfile.Profile()
         pr.enable()
     ms_dev, wall_dev, launches, ndet = timed(dev_batches, args.steps)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(last["out"], Path(args.dump_outputs))
     if args.profile_host:
         pr.disable()
         pstats.Stats(pr, stream=sys.stderr).sort_stats("cumulative").print_stats(35)
@@ -580,17 +632,9 @@ def main():
         achieved = d["flops"] / (d["ms"] / 1e3) / 1e12
         conv_ms = sum(v["ms"] for k, v in per_kernel.items() if k.startswith("conv"))
         conv_fl = sum(v["flops"] for k, v in per_kernel.items() if k.startswith("conv"))
-        traffic = None
-        for cand in ("r02_tracknet_dram_bytes.json", "r01_tracknet_dram_bytes.json"):
-            tf = ROOT / "profiles" / cand
-            if tf.exists() and dom == "conv_halo_kernel" and ball is not None:
-                traffic = json.loads(tf.read_text())
-                break
         roof = {"bound": "tensor", "kernel": dom, "achieved": round(achieved, 1), "peak": pk["tflops_sustained"],
-                "peak_kind": f"{pk['source']} cuBLAS bf16 sustained (fp16 runs at the same tensor-core rate)",
+                "peak_kind": f"{pk['source']} fp16 dense tensor-core rate",
                 "unit": "TFLOP/s", "frac": round(achieved / pk["tflops_sustained"], 4),
-                "traffic": (traffic or {}).get("dram_gb_per_step_tracknet_halo_launches"),
-                "traffic_note": (traffic or {}).get("note"),
                 "launches_per_step": d["launches"], "kernel_ms_per_step": round(d["ms"], 3),
                 "timing": "median of 5 per-op CUDA-event timings",
                 "algorithmic_gflop_per_step": round(d["flops"] / 1e9, 1),

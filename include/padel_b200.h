@@ -1,5 +1,5 @@
 /*
- * padel_b200.h — C ABI of libpadel_b200.so: the B200 (sm_100a) per-frame inference engine that replaces the
+ * padel_b200.h — C ABI of libpadel_b200.so: the H100 (sm_90a) per-frame inference engine that replaces the
  * model forwards of the four padel_analytics trackers.
  *
  * The reference (pure Python) has no FFI; its "plugin boundary" is the duck-typed model object each tracker holds:
@@ -58,7 +58,7 @@ int pb_version(void);
 /* Number of kernels this library has launched since load (bench.py's gpu_launches). */
 long long pb_launch_count(void);
 
-/* ---- fused conv + bias + activation (+ residual) : implicit GEMM on tcgen05 tensor cores ------------------
+/* ---- fused conv + bias + activation (+ residual) : implicit GEMM on wgmma tensor cores ------------------
  * Replaces ultralytics Conv (Conv2d+BN+SiLU, BN folded) and TrackNet Conv2DBlock (models.py:5-17).          */
 typedef struct pb_conv_desc {
   const void* in;  /* half NHWC (N,H,W,C); for in_layout == PB_IN_STEM4 see below */

@@ -1,2 +1,2 @@
-"""padel_analytics_b200 — B200-native (sm_100a) inference engine for the padel_analytics tracker hot path."""
+"""padel_analytics_b200 — H100-native (sm_90a) inference engine for the padel_analytics tracker hot path."""
 __version__ = "0.1.0"

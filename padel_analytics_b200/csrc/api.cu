@@ -36,7 +36,7 @@ static int device_sms() {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess ||
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
-      sms = 148;
+      sms = 132;  // H100 SXM
   });
   return sms;
 }

@@ -33,11 +33,11 @@ __device__ __forceinline__ void bias_act16(const uint32_t (&r)[16], const float*
   }
 }
 
-// 32-byte store (STG.256): one instruction and one full 32-byte sector per 16 fp16 channels
+// one 32-byte run of 16 fp16 channels (a full 32-byte sector) as two 16-byte stores
 __device__ __forceinline__ void st_global_256(void* p, const uint4& a, const uint4& b) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(a.x), "r"(a.y), "r"(a.z),
-               "r"(a.w), "r"(b.x), "r"(b.y), "r"(b.z), "r"(b.w)
-               : "memory");
+  uint4* q = reinterpret_cast<uint4*>(p);
+  q[0] = a;
+  q[1] = b;
 }
 
 struct EpiPix {
@@ -140,9 +140,7 @@ __device__ __forceinline__ void epilogue_store16(const ConvKParams& kp, const Ep
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// Fast epilogue for the common case (fp16 NHWC slice out, 32-byte aligned 16-channel runs, no fused head):
-// software-pipelined over 16-column chunks -- the tcgen05.ld (and the residual loads) of chunk i+1 are in flight
-// while chunk i is activated, packed and stored -- and across the S sub-tiles of a halo tile.
+// Fast epilogue for the common case (fp16 NHWC slice out, 32-byte aligned 16-channel runs, no fused head).
 // ------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ bool epilogue_fast_ok(const ConvKParams& kp) {
   if ((kp.dbg_flags & 2) != 0 && kp.out2_mode == PB_OUT2_NONE) return false;
@@ -155,10 +153,9 @@ __device__ __forceinline__ bool epilogue_fast_ok(const ConvKParams& kp) {
 }
 
 // SiLU on four values with ONE reciprocal: 1/da = db*dc*dd * r, ... with r = 1/(da*db*dc*dd), d = 1 + 2^(-v*log2 e).
-// The fast epilogue of a wide SiLU layer is bound by the XU (MUFU) pipe -- ncu on the pose head conv 64->192 @160^2:
-// sm__inst_executed_pipe_xu_realtime 75 %, every other pipe < 45 % (profiles/r02_ncu_yolo.md) -- and the plain form
-// v / (1 + exp(-v)) costs two MUFU operations per value (EX2 + RCP); this one costs 1.25 plus a few FMULs on the
-// idle FMA pipe, with the same few-ulp fp32 accuracy (no approximation of the function itself).
+// The plain form v / (1 + exp(-v)) costs two MUFU operations per value (EX2 + RCP), and the MUFU pipe is what bounds
+// the epilogue of a wide SiLU layer; this one costs 1.25 plus a few FMULs on the FMA pipe, with the same few-ulp fp32
+// accuracy (no approximation of the function itself).
 // The exponent is clamped to 2^30 so that the product of four stays finite (< 2^121); silu(v) for v < -20.8 is below
 // 2e-8 in magnitude either way, i.e. an fp16 zero / smallest subnormal.
 // PADEL_B200_CONV_DEBUG bit 0 selects the plain two-MUFU form for A/B runs.
@@ -196,8 +193,8 @@ __device__ __forceinline__ void epi_add_res16(const uint4 (&rv)[2], float (&v)[1
     for (int j = 0; j < 4; ++j) {
       const float2 f = __half22float2(h2[j]);
       // __fadd_rn: never contracted with the activation's last multiply into an FMA -- the folded epilogue classes
-      // would otherwise round differently from the run-time epilogue (which the CTA-pair kernels use), and a frame's
-      // result must not depend on which of them its batch size selects (tests/test_full_size_gpu.py)
+      // would otherwise round differently from the run-time epilogue, and a frame's result must not depend on which
+      // of them its batch size selects (tests/test_full_size_gpu.py)
       v[8 * g + 2 * j] = __fadd_rn(v[8 * g + 2 * j], f.x);
       v[8 * g + 2 * j + 1] = __fadd_rn(v[8 * g + 2 * j + 1], f.y);
     }
@@ -299,87 +296,180 @@ __device__ __forceinline__ void epi_chunk(int act, int has_res, bool plain_silu,
   }
 }
 
-// One thread's share of a tile: `S` sub-tiles (accumulator sets `sub_cols` TMEM columns apart, pixels `sub_out` /
-// `sub_res` BYTES / halves apart in the output / residual tensors), `nch` 16-column chunks each (`cout_n` channels of
-// this N tile exist).  valid_mask bit j = the thread's pixel of sub-tile j exists.  op0 / rp0 point at channel 0 of
-// this N tile.  Software pipeline: the tcgen05.ld of chunk i+1 is in flight while chunk i is processed.
-// kEpi (a kernel template parameter, chosen per plan by the host -- conv_epi_class): 0 = every case at run time;
-// PB_EPI_SILU / PB_EPI_RELU = the plain case (that activation, no residual, fp16 NHWC store, no secondary output),
-// PB_EPI_SILU_RES = SiLU then the shortcut add, PB_EPI_F32 = the linear fp32 head outputs, with everything folded at
-// compile time.  The epilogue warps of the light layers are issue-latency-bound (two epilogue warps
-// per SM sub-partition; profiles/r02_epilogue_stalls.md) and the run-time form spends 14 of its ~285 instructions per
-// chunk on CTA-uniform branches.  One epilogue per kernel instantiation: a kernel holding several copies exceeds the
-// 128-register budget and spills (measured; same note).
-template <int kEpi>
-__device__ __forceinline__ void epilogue_fast(const ConvKParams& kp, const EpiOut& eo_in, uint32_t t_addr0, int S,
-                                              uint32_t sub_cols, int nch, int cout_n, const float* __restrict__ sbias,
-                                              char* op0, const __half* rp0, size_t sub_out, size_t sub_res,
-                                              uint32_t valid_mask, char* op20 = nullptr, size_t sub_out2 = 0) {
-  uint32_t ra[16], rb[16];
-  constexpr bool kSpec = kEpi != PB_EPI_GENERIC;
-  EpiOut eo = eo_in;
-  if (kSpec) {
-    eo.mode = kEpi == PB_EPI_F32 ? PB_OUT_F32_NHWC : PB_OUT_F16_NHWC;
-    eo.mode2 = PB_OUT2_NONE;
+// Epilogue of the wgmma conv kernels.  A consumer warp holds 16 pixels x N columns of each sub-tile in the wgmma
+// fragment layout; per 32-column chunk a shared-memory scratch transposes them so that lane l gets 16 channels of one
+// pixel (row l % 16, columns 16 (l / 16) ..), the unit of the stores above (lanes l ^ 1 / l ^ 8: the neighbours the
+// PB_OUT2_POOL2 butterfly needs).  Sub-tile j occupies acc[j * 16 ceil(N / 32) ...): chunk u is acc[16 u .. 16 u + 16).
+constexpr int kConvAccRegs = 128;   // fp32 accumulators per consumer thread: S * 16 * ceil(N / 32) <= 128
+constexpr int kEpiScratchPitch = 36;  // floats per scratch row (32 + 4 spreads the fragment stores over the banks)
+constexpr int kEpiScratchFloats = 16 * kEpiScratchPitch;  // per consumer warp
+
+template <int kU>
+__device__ __forceinline__ void epi_frag_store(const float (&acc)[kConvAccRegs], float* scr, int lane) {
+  const int r0 = lane >> 2, q = lane & 3;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    *reinterpret_cast<float2*>(scr + r0 * kEpiScratchPitch + 8 * i + 2 * q) =
+        make_float2(acc[16 * kU + 4 * i], acc[16 * kU + 4 * i + 1]);
+    *reinterpret_cast<float2*>(scr + (r0 + 8) * kEpiScratchPitch + 8 * i + 2 * q) =
+        make_float2(acc[16 * kU + 4 * i + 2], acc[16 * kU + 4 * i + 3]);
   }
-  const int act = (kEpi == PB_EPI_SILU || kEpi == PB_EPI_SILU_RES) ? PB_ACT_SILU
-                  : kEpi == PB_EPI_RELU                            ? PB_ACT_RELU
-                  : kEpi == PB_EPI_F32                             ? PB_ACT_NONE
-                                                                   : kp.act;
-  const int has_res = kEpi == PB_EPI_SILU_RES ? 1 : kSpec ? 0 : (kp.res != nullptr ? (kp.res_first ? 2 : 1) : 0);
-  const bool plain_silu = kSpec ? false : (kp.dbg_flags & 1) != 0;
-  const int cbytes = eo.mode == PB_OUT_F32_NHWC ? 64 : 32;  // bytes of one 16-channel chunk in the output
-  int j = 0, c = 0;
-  tmem_ld16(t_addr0, ra);
-  // the shortcut operand is fetched one chunk ahead, like the accumulator: a global load issued and consumed inside
-  // the same chunk would put its whole latency on the chunk's critical path
-  constexpr bool kPrefetchRes = kEpi == PB_EPI_SILU_RES;  // (the run-time epilogue has no registers to spare for it)
-  uint4 rva[2] = {}, rvb[2] = {};
-  if (kPrefetchRes && (valid_mask & 1u)) {
-    const uint4* rp = reinterpret_cast<const uint4*>(rp0);
-    rva[0] = __ldg(rp);
-    rva[1] = __ldg(rp + 1);
-  }
-#define PB_EPI_STAGE(cur, nxt, rvc, rvn)                                                                \
-  {                                                                                                     \
-    int jn = j, cn = c + 1;                                                                             \
-    if (cn == nch) {                                                                                    \
-      cn = 0;                                                                                           \
-      ++jn;                                                                                             \
-    }                                                                                                   \
-    const bool more = jn < S;                                                                           \
-    const bool valid = ((valid_mask >> j) & 1u) != 0;                                                   \
-    if (kPrefetchRes) {                                                                                 \
-      if (more && ((valid_mask >> jn) & 1u)) {                                                          \
-        const uint4* rp = reinterpret_cast<const uint4*>(rp0 + (size_t)jn * sub_res + cn * 16);         \
-        rvn[0] = __ldg(rp);                                                                             \
-        rvn[1] = __ldg(rp + 1);                                                                         \
-      }                                                                                                 \
-    }                                                                                                   \
-    uint4 rvl[2] = {};                                                                                  \
-    if (!kPrefetchRes && has_res && valid) { /* consumed after the activation math of this chunk */     \
-      const uint4* rp = reinterpret_cast<const uint4*>(rp0 + (size_t)j * sub_res + c * 16);             \
-      rvl[0] = __ldg(rp);                                                                               \
-      rvl[1] = __ldg(rp + 1);                                                                           \
-    }                                                                                                   \
-    tmem_ld_wait16(cur);                                                                                \
-    if (more) tmem_ld16(t_addr0 + (uint32_t)jn * sub_cols + (uint32_t)(cn * 16), nxt);                  \
-    epi_chunk(act, has_res, plain_silu, eo, cur, sbias + c * 16, op0 + (size_t)j * sub_out + (size_t)(c * cbytes), kPrefetchRes ? rvc : rvl, valid, \
-              cout_n - c * 16, op20 + (size_t)j * sub_out2 + (size_t)(c * 32), kEpi == PB_EPI_F32);      \
-    if (!more) break;                                                                                   \
-    j = jn;                                                                                             \
-    c = cn;                                                                                             \
-  }
-  for (;;) {
-    PB_EPI_STAGE(ra, rb, rva, rvb)
-    PB_EPI_STAGE(rb, ra, rvb, rva)
-  }
-#undef PB_EPI_STAGE
 }
 
-// Two alternative store paths were built and measured on B200 and then removed (profiles/r02_exp_epilogue.md): a
-// shared-memory transposition so that every store instruction covers full 128-byte lines (slower on every layer), and
-// a TMA bulk-store epilogue (cp.async.bulk.tensor from a swizzled smem tile: 34/34 correctness cases pass, no gain on
-// any program, and merely compiling it in cost the product kernels 20 % through register pressure).
+// chunk u of the accumulators -> this lane's 16 channels
+__device__ __forceinline__ void epi_transpose16(const float (&acc)[kConvAccRegs], int u, float* scr, int lane,
+                                                uint32_t (&r)[16]) {
+  __syncwarp();  // the previous chunk's reads are done
+  switch (u) {  // CTA-uniform; the accumulator index has to be a compile-time constant
+    case 0: epi_frag_store<0>(acc, scr, lane); break;
+    case 1: epi_frag_store<1>(acc, scr, lane); break;
+    case 2: epi_frag_store<2>(acc, scr, lane); break;
+    case 3: epi_frag_store<3>(acc, scr, lane); break;
+    case 4: epi_frag_store<4>(acc, scr, lane); break;
+    case 5: epi_frag_store<5>(acc, scr, lane); break;
+    case 6: epi_frag_store<6>(acc, scr, lane); break;
+    default: epi_frag_store<7>(acc, scr, lane); break;
+  }
+  __syncwarp();
+  const float4* src = reinterpret_cast<const float4*>(scr + (lane & 15) * kEpiScratchPitch + 16 * (lane >> 4));
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const float4 f = src[k];
+    r[4 * k + 0] = __float_as_uint(f.x);
+    r[4 * k + 1] = __float_as_uint(f.y);
+    r[4 * k + 2] = __float_as_uint(f.z);
+    r[4 * k + 3] = __float_as_uint(f.w);
+  }
+}
+
+// One lane's 16 channels (column `col` of N tile `nt`) of pixel px.  kEpi (chosen per plan, conv_epi_class): generic
+// (run time), or a plain class -- SiLU / ReLU / SiLU + shortcut / fp32 head -- folded at compile time.
+template <int kEpi>
+__device__ __forceinline__ void epi_unit(const ConvKParams& kp, const EpiPix& px, bool pool_writer, int nt, int col,
+                                         uint32_t (&r)[16], const float* __restrict__ sbias, bool fast,
+                                         float (&hacc)[8]) {
+  constexpr bool kSpec = kEpi != PB_EPI_GENERIC;
+  const int ch = nt * kp.BN + col;  // output channel of r[0]
+  int cout_n = kp.cout_store - nt * kp.BN;  // channels of this N tile that exist
+  cout_n = cout_n < kp.BN ? cout_n : kp.BN;
+  const bool exists = col < cout_n;
+  if (fast) {
+    const int act = (kEpi == PB_EPI_SILU || kEpi == PB_EPI_SILU_RES) ? PB_ACT_SILU
+                    : kEpi == PB_EPI_RELU                            ? PB_ACT_RELU
+                    : kEpi == PB_EPI_F32                             ? PB_ACT_NONE
+                                                                     : kp.act;
+    const int has_res = kEpi == PB_EPI_SILU_RES ? 1 : kSpec ? 0 : (kp.res != nullptr ? (kp.res_first ? 2 : 1) : 0);
+    const bool plain_silu = kSpec ? false : (kp.dbg_flags & 1) != 0;
+    EpiOut eo;
+    eo.mode = kSpec ? (kEpi == PB_EPI_F32 ? PB_OUT_F32_NHWC : PB_OUT_F16_NHWC) : kp.out_mode;
+    eo.mode2 = kSpec ? PB_OUT2_NONE : kp.out2_mode;
+    eo.pool_writer = pool_writer;
+    eo.dx = eo.dy = eo.dx2 = eo.dy2 = 0;
+    const size_t esz = eo.mode == PB_OUT_F32_NHWC ? 4 : 2;
+    const size_t pxb = (size_t)kp.out_C * esz;  // bytes per output pixel
+    const size_t up_pix = ((size_t)px.n * (2 * kp.Ho) + 2 * px.oh) * (2 * kp.Wo) + 2 * px.ow;
+    size_t opix = px.pix;
+    if (eo.mode == PB_OUT_F16_NHWC_UP2) {
+      opix = up_pix;
+      eo.dx = pxb;
+      eo.dy = (size_t)(2 * kp.Wo) * pxb;
+    }
+    char* op = reinterpret_cast<char*>(kp.out) + opix * pxb + (size_t)(kp.out_coff + ch) * esz;
+    char* op2 = nullptr;
+    if (eo.mode2 != PB_OUT2_NONE) {
+      const size_t pxb2 = (size_t)kp.out2_C * 2;
+      size_t pix2;
+      if (eo.mode2 == PB_OUT2_UP2) {
+        pix2 = up_pix;
+        eo.dx2 = pxb2;
+        eo.dy2 = (size_t)(2 * kp.Wo) * pxb2;
+      } else {  // POOL2 (Ho, Wo even): the pooled pixel of the window whose top-left corner this lane holds
+        pix2 = ((size_t)px.n * (kp.Ho >> 1) + (px.oh >> 1)) * (kp.Wo >> 1) + (px.ow >> 1);
+      }
+      op2 = reinterpret_cast<char*>(kp.out2) + pix2 * pxb2 + (size_t)(kp.out2_coff + ch) * 2;
+    }
+    const bool valid = px.valid && exists;
+    uint4 rv[2] = {};
+    if (has_res && valid) {
+      const uint4* rp = reinterpret_cast<const uint4*>(kp.res + px.pix * kp.res_C + kp.res_coff + ch);
+      rv[0] = __ldg(rp);
+      rv[1] = __ldg(rp + 1);
+    }
+    epi_chunk(act, has_res, plain_silu, eo, r, sbias + col, op, rv, valid, cout_n - col, op2, kEpi == PB_EPI_F32);
+  } else if constexpr (kEpi == PB_EPI_GENERIC) {
+    if (px.valid && exists) {
+      float v[16];
+      bias_act16(r, sbias + col, kp.act, v,
+                 (kp.res && kp.res_first) ? kp.res + px.pix * kp.res_C + kp.res_coff + ch : nullptr);
+      epilogue_store16(kp, px, ch, col, v, hacc);
+    }
+  }
+}
+
+// One consumer warp's tile; pix_of(j, pool_writer) = this lane's pixel in sub-tile j.  Every lane runs every chunk
+// (the butterfly shuffles); the fused head adds the half-pixel sums of lanes l and l ^ 16.
+template <int kEpi, typename PixOf>
+__device__ __forceinline__ void epilogue_tile(const ConvKParams& kp, const float (&acc)[kConvAccRegs], int S, int nt,
+                                              const float* __restrict__ sbias, float* scr, int lane, PixOf pix_of) {
+  const int nch = (kp.BN + 31) >> 5;
+  const bool fast = kEpi != PB_EPI_GENERIC || epilogue_fast_ok(kp);  // the host picks a plain class only when it holds
+  const int col0 = 16 * (lane >> 4);
+  for (int j = 0; j < S; ++j) {
+    bool pool_writer = false;
+    const EpiPix px = pix_of(j, pool_writer);
+    float hacc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};  // fused 1x1 head partial sums
+    for (int c = 0; c < nch; ++c) {
+      uint32_t r[16];
+      epi_transpose16(acc, j * nch + c, scr, lane, r);
+      epi_unit<kEpi>(kp, px, pool_writer, nt, 32 * c + col0, r, sbias, fast, hacc);
+    }
+    if (kEpi == PB_EPI_GENERIC && !fast && kp.head_n > 0) {
+#pragma unroll
+      for (int q = 0; q < 8; ++q) hacc[q] += __shfl_xor_sync(0xffffffffu, hacc[q], 16);
+      if (lane < 16 && px.valid) {
+        const size_t plane = (size_t)kp.Ho * kp.Wo;
+        float* ho = kp.head_out + (size_t)px.n * kp.head_n * plane + (size_t)px.oh * kp.Wo + px.ow;
+#pragma unroll
+        for (int q = 0; q < 8; ++q)
+          if (q < kp.head_n) ho[(size_t)q * plane] = __fdividef(1.f, 1.f + __expf(-(hacc[q] + __ldg(kp.head_b + q))));
+      }
+    }
+  }
+}
+
+// acc (+)= A * B^T over kSteps k-steps of 16 for the warpgroup's 64 rows of kS sub-tiles (A descriptors sub_units
+// apart); accum = 0 overwrites.  kN = the N tile, a compile-time constant of the instruction.
+template <int kN, int kS, int kSteps>
+__device__ __forceinline__ void mma_n(float (&acc)[kConvAccRegs], uint64_t ad, uint64_t sub_units, uint64_t bd,
+                                      uint32_t accum) {
+  constexpr int kAS = (kN + 31) / 32 * 16;
+  if constexpr (kS * kAS <= kConvAccRegs) {
+#pragma unroll
+    for (int j = 0; j < kS; ++j)
+#pragma unroll
+      for (int k = 0; k < kSteps; ++k)
+        wgmma_f16<kN>(acc + j * kAS, ad + (uint64_t)j * sub_units + (uint64_t)(2 * k), bd + (uint64_t)(2 * k),
+                      k == 0 ? accum : 1u);
+  }
+}
+template <int kS, int kSteps>
+__device__ __forceinline__ void mma_group(int n, float (&acc)[kConvAccRegs], uint64_t ad, uint64_t sub_units,
+                                          uint64_t bd, uint32_t accum) {
+  switch (n) {  // CTA-uniform
+#define PB_MMA_CASE(n_) \
+  case n_: mma_n<n_, kS, kSteps>(acc, ad, sub_units, bd, accum); break;
+    PB_MMA_CASE(16) PB_MMA_CASE(32) PB_MMA_CASE(48) PB_MMA_CASE(64) PB_MMA_CASE(80) PB_MMA_CASE(96)
+    PB_MMA_CASE(112) PB_MMA_CASE(128) PB_MMA_CASE(144) PB_MMA_CASE(160) PB_MMA_CASE(176) PB_MMA_CASE(192)
+    PB_MMA_CASE(208) PB_MMA_CASE(224) PB_MMA_CASE(240) PB_MMA_CASE(256)
+#undef PB_MMA_CASE
+    default: break;
+  }
+}
+
+// Consumer warps release a shared-memory slot once their wgmmas reading it have completed (one arrive per warp).
+__device__ __forceinline__ void consumer_release(uint64_t* bar, int lane) {
+  __syncwarp();
+  if (lane == 0) mbar_arrive(bar);
+}
 
 }  // namespace pb

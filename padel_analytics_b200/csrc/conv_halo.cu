@@ -2,14 +2,13 @@
 // shared-memory halo tile per 64(32/16)-channel block.
 //
 // Why: with one TMA box per tap (conv_tc_kernel) every K-block of a small-N layer moves 16 KB of activations for
-// four UMMAs and the kernel is bound by L2->SM / TMA delivery (measured 0.35-0.43 PFLOP/s on TrackNet's N=64
-// layers).  Here the CTA tile is 16 rows x (8*S) columns of output pixels = S sub-tiles of M=128; its
+// four k-steps of MMAs, and the kernel is bound by L2->SM / TMA delivery on TrackNet's N=64 layers.  Here the CTA tile is 16 rows x (8*S) columns of output pixels = S sub-tiles of M=128; its
 // (16+2) x (8*S+2) pixel halo is fetched by a single TMA box, and tap (r,s) of sub-tile j is just a different
-// UMMA descriptor over the same bytes:
+// wgmma descriptor over the same bytes:
 //     start = halo + ((r*P + 8*j + s) * row_bytes),   SBO (8-row group stride) = P * row_bytes,   P = 8*S + 2
 // (one 8-row group = 8 horizontally adjacent pixels, consecutive groups = consecutive image rows).  This relies on
-// tcgen05 applying the 128/64/32-byte swizzle XOR on absolute shared-memory address bits, which
-// scripts/exp_umma_shift.py verified on B200 (descriptor base_offset = 0 is exact for any row shift / any SBO).
+// the tensor core applying the 128/64/32-byte swizzle XOR on absolute shared-memory address bits (descriptor base
+// offset 0 for any row shift / any SBO); tests/test_conv_gpu.py checks every halo variant against torch.
 // Weights are fetched per (channel block, tap group) by a second producer warp and shared by the S sub-tile MMAs.
 //
 // Replaces the same reference layers as conv_tc.cu (TrackNet Conv2DBlock models.py:5-17; ultralytics 3x3 convs).
@@ -31,43 +30,25 @@ struct HaloSmemTail {
   uint64_t a_empty[kHaloMaxA];
   uint64_t b_full[kHaloMaxB];
   uint64_t b_empty[kHaloMaxB];
-  uint64_t tmem_full[kConvMaxAcc];
-  uint64_t tmem_empty[kConvMaxAcc];
-  uint32_t tmem_base;
-  uint32_t pad_[3];
   float bias[kConvMaxCout];
+  float scratch[kConvConsumerWarps * kEpiScratchFloats];  // epilogue transposition, one slice per consumer warp
 };
 
 struct HaloTile {
   int tw, th, n;
 };
-// pair mode: a "tile" is two vertically adjacent 16-row tiles, one per CTA of the pair (crank = 0 / 1)
-__device__ __forceinline__ HaloTile halo_decode(const ConvKParams& kp, int tile, uint32_t crank) {
+__device__ __forceinline__ HaloTile halo_decode(const ConvKParams& kp, int tile) {
   HaloTile t;
-  int q, th;
+  int q;
   fast_divmod(q, t.tw, tile, kp.fd_w);
-  fast_divmod(t.n, th, q, kp.fd_h);
-  t.th = kp.pair ? th * 2 + (int)crank : th;
+  fast_divmod(t.n, t.th, q, kp.fd_h);
   return t;
 }
 
-// row_bytes 128 / 64 / 32: the swizzled K-major layouts.  row_bytes 16: the un-swizzled K-major layout -- 8-row core
-// matrices of 16-byte rows at a 16-byte pitch, 8-row groups `sbo_bytes` apart, the second 16-byte half of a K = 16 row
-// `lbo_bytes` further (16: the row that follows -- overlapping rows, used by the stem's raw-pixel operand; the roles of
-// LBO and SBO in this layout were confirmed on hardware: swapping them fails tests/test_conv_gpu.py::test_stem_*).
-__device__ __forceinline__ uint64_t umma_desc_sbo(uint32_t saddr, uint32_t row_bytes, uint32_t sbo_bytes,
-                                                  uint32_t lbo_bytes = 16) {
-  const uint64_t layout = row_bytes == 128 ? 2ull : (row_bytes == 64 ? 4ull : (row_bytes == 32 ? 6ull : 0ull));
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) |
-         (1ull << 46) | (layout << 61);
-}
-
-// kPair is a compile-time switch: a kernel that contains cta_group::2 instructions can only be launched as a
-// cluster of two, so the single-CTA and the CTA-pair variants are separate instantiations.
-// kS (sub-tiles) and kSteps (16-element k-steps per channel block) are compile-time so the UMMA issue
-// loop is straight-line code with immediate descriptor offsets.
-template <bool kPair, int kS, int kSteps, int kEpi>
-__global__ void __launch_bounds__(kConvMaxThreads, 1)
+// kS (sub-tiles) and kSteps (16-element k-steps per channel block) are compile-time so the wgmma issue loop is
+// straight-line code with immediate descriptor offsets.
+template <int kS, int kSteps, int kEpi>
+__global__ void __launch_bounds__(kConvThreads, 1)
 conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
                  const __grid_constant__ ConvKParams kp) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -78,112 +59,64 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  // bring-up timeline (libpadel_b200_debug.so only: kp.dbg is NULL in the product build): GPU-wide nanosecond stamps of
-  // the first and the last CTA -- entry, after griddepcontrol.wait, exit -- to see how consecutive layers overlap
-  const bool gdbg = kp.dbg != nullptr && threadIdx.x == 0 && (blockIdx.x == 0 || blockIdx.x == gridDim.x - 1);
-  long long* gslot = kp.dbg + (3 * 64 + (blockIdx.x == 0 ? 0 : 1)) * 4;
-  if (gdbg) gslot[0] = (long long)globaltimer_ns();
   constexpr int S = kS;
   const int G = kp.hs_G;
   const uint32_t row_bytes = (uint32_t)kp.KB * 2u;       // weight rows (and activation rows unless stride 2)
   const uint32_t a_row_bytes = kp.hs_a_row_bytes;        // activation (halo) rows
   const int tap_groups = kp.hs_ntaps / G;
-  // CTA-pair mode (cluster of 2, cta_group::2): both CTAs load their own halo and half of the weights, the even
-  // CTA issues M=256 UMMAs over both, so every SM reads only half of B from its shared memory.
-  constexpr int pair = kPair ? 1 : 0;
-  const uint32_t crank = pair ? cluster_ctarank() : 0u;
-  const int cta0 = pair ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int cstride = pair ? (int)(gridDim.x >> 1) : (int)gridDim.x;
 
-  if (warp == 0 && lane == 0) tma_prefetch_desc(&tmap_a);
-  if (warp == 6 && lane == 0) tma_prefetch_desc(&tmap_w);
-  if (warp == 1 && lane == 0) {
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&tmap_a);
     for (int i = 0; i < kp.a_stages; ++i) {
       mbar_init(&tail->a_full[i], 1);
-      mbar_init(&tail->a_empty[i], 1);
+      mbar_init(&tail->a_empty[i], kConvConsumerWarps);
     }
     for (int i = 0; i < kp.b_stages; ++i) {
       mbar_init(&tail->b_full[i], 1);
-      mbar_init(&tail->b_empty[i], 1);
-    }
-    for (int i = 0; i < kp.acc_stages; ++i) {
-      mbar_init(&tail->tmem_full[i], 1);
-      mbar_init(&tail->tmem_empty[i], pair ? 8 : 4);  // one arrive per epilogue warp (of both CTAs in pair mode)
+      mbar_init(&tail->b_empty[i], kConvConsumerWarps);
     }
     fence_mbar_init();
   }
-  if (warp == 2) {
-    if (pair) {
-      tmem_alloc2(&tail->tmem_base, (uint32_t)kp.tmem_cols);
-      tmem_relinquish2();
-    } else {
-      tmem_alloc(&tail->tmem_base, (uint32_t)kp.tmem_cols);
-      tmem_relinquish();
-    }
-  }
+  if (warp == 1 && lane == 0) tma_prefetch_desc(&tmap_w);
   for (int i = threadIdx.x; i < kp.cout_pad; i += blockDim.x) tail->bias[i] = kp.bias[i];
-  tc_fence_before();
   __syncthreads();
-  if (pair) cluster_sync_all();  // the peer's barriers must be initialised before anything arrives on them
-  tc_fence_after();
-  const uint32_t tmem_base = tail->tmem_base;
   // PDL: the prologue above touched constant data only; from here on activations are read and written.  The weight
-  // producer (warp 6) reads constants only and starts fetching while the previous kernel is still running.
+  // producer (warp 1) reads constants only and starts fetching while the previous kernel is still running.
   griddep_launch_dependents();
-  if (warp != 6) griddep_wait();
-  if (gdbg) gslot[1] = (long long)globaltimer_ns();
+  if (warp != 1) griddep_wait();
 
-  if (warp == 0) {
-    // ===================== halo producer: one TMA box per (tile, channel block) =====================
-    if (lane == 0) {
+  if (warp < 4) {
+    warpgroup_reg_dealloc<kConvProducerRegs>();
+    if (warp == 0 && lane == 0) {
+      // ===================== halo producer: one TMA box per (tile, channel block) =====================
       int st = 0;
       uint32_t ph = 0;
-      int seq = -1;
-      for (int tile = cta0; tile < kp.total_tiles; tile += cstride) {
-        const HaloTile t = halo_decode(kp, tile, crank);
-        ++seq;
-        const bool dbg = kp.dbg != nullptr && blockIdx.x == 0 && seq < 64;
-        if (dbg) kp.dbg[(0 * 64 + seq) * 4 + 0] = clock64();
+      for (int tile = blockIdx.x; tile < kp.total_tiles; tile += gridDim.x) {
+        const HaloTile t = halo_decode(kp, tile);
         for (int cb = 0; cb < kp.kblocks; ++cb) {
           mbar_wait(&tail->a_empty[st], ph ^ 1);
-          if (dbg && cb == 0) kp.dbg[(0 * 64 + seq) * 4 + 1] = clock64();
-          if (pair) {
-            if (crank == 0) mbar_arrive_expect_tx(&tail->a_full[st], 2u * kp.halo_bytes);  // both CTAs' halos
-            tma_load_5d_2sm(a_base + (size_t)st * kp.a_bytes, &tmap_a, &tail->a_full[st], kp.c_in_off + cb * kp.KB,
-                            t.tw * 8 * S + kp.hs_x0, 0, t.th * 16 + kp.hs_y0, t.n);
-          } else {
-            mbar_arrive_expect_tx(&tail->a_full[st], kp.halo_bytes);
-            tma_load_5d(a_base + (size_t)st * kp.a_bytes, &tmap_a, &tail->a_full[st], kp.c_in_off + cb * kp.KB,
-                        t.tw * 8 * S + kp.hs_x0, 0, t.th * 16 + kp.hs_y0, t.n);
-          }
+          mbar_arrive_expect_tx(&tail->a_full[st], kp.halo_bytes);
+          tma_load_5d(a_base + (size_t)st * kp.a_bytes, &tmap_a, &tail->a_full[st], kp.c_in_off + cb * kp.KB,
+                      t.tw * 8 * S + kp.hs_x0, 0, t.th * 16 + kp.hs_y0, t.n);
           if (++st == kp.a_stages) {
             st = 0;
             ph ^= 1;
           }
         }
       }
-    }
-    __syncwarp();
-  } else if (warp == 6) {
-    // ===================== weight producer: one TMA box per (channel block, tap group) =====================
-    // Resident mode (kp.b_resident: the whole filter bank fits next to the halo ring): every box is fetched ONCE per
-    // CTA and reused by all its tiles -- without it a small-channel layer re-reads its weights from L2 for every
-    // tile, as many bytes as the activations themselves.
-    if (lane == 0) {
+    } else if (warp == 1 && lane == 0) {
+      // ===================== weight producer: one TMA box per (channel block, tap group) =====================
+      // Resident mode (kp.b_resident: the whole filter bank fits next to the halo ring): every box is fetched ONCE per
+      // CTA and reused by all its tiles -- without it a small-channel layer re-reads its weights from L2 for every
+      // tile, as many bytes as the activations themselves.
       int st = 0;
       uint32_t ph = 0;
-      for (int tile = cta0; tile < kp.total_tiles; tile += cstride) {
+      for (int tile = blockIdx.x; tile < kp.total_tiles; tile += gridDim.x) {
         for (int cb = 0; cb < kp.kblocks; ++cb) {
           for (int tg = 0; tg < tap_groups; ++tg) {
             if (!kp.b_resident) mbar_wait(&tail->b_empty[st], ph ^ 1);
-            if (pair) {  // each CTA fetches its half of the output channels
-              if (crank == 0) mbar_arrive_expect_tx(&tail->b_full[st], 2u * kp.b_tx_bytes);
-              tma_load_3d_2sm(b_base + (size_t)st * kp.b_bytes, &tmap_w, &tail->b_full[st], cb * kp.KB,
-                              (int)crank * (kp.BN / 2), tg * G);
-            } else {
-              mbar_arrive_expect_tx(&tail->b_full[st], kp.b_tx_bytes);
-              tma_load_3d(b_base + (size_t)st * kp.b_bytes, &tmap_w, &tail->b_full[st], cb * kp.KB, 0, tg * G);
-            }
+            mbar_arrive_expect_tx(&tail->b_full[st], kp.b_tx_bytes);
+            tma_load_3d(b_base + (size_t)st * kp.b_bytes, &tmap_w, &tail->b_full[st], cb * kp.KB, 0, tg * G);
             if (++st == kp.b_stages) {
               st = 0;
               ph ^= 1;
@@ -193,209 +126,68 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         if (kp.b_resident) break;
       }
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ===================== UMMA issuer (pair mode: the even CTA only) =====================
-    // All 32 lanes run the loops on warp-uniform values; only the elected lane's tcgen05 instructions take effect.
-    if (crank == 0) {
-      const uint32_t lead = elect_one();
-      const uint32_t tm_base = __shfl_sync(0xffffffffu, tmem_base, 0);
-      int ast = 0, bst = 0, acc = 0;
-      uint32_t aph = 0, bph = 0, acc_ph = 0;
-      const uint32_t sbo = (uint32_t)kp.hs_sbo_rows * a_row_bytes;
-      const uint32_t tap_b_units = ((uint32_t)(pair ? kp.BN / 2 : kp.BN) * row_bytes) >> 4;  // 16-byte units
-      const uint64_t sub_units = (uint64_t)((8u * a_row_bytes) >> 4);                          // next sub-tile: +8 pixels
-      const uint32_t acc_cols = (uint32_t)kp.acc_cols;
-      const uint32_t idesc = kp.idesc;
-      int seq = -1;
-      for (int tile = cta0; tile < kp.total_tiles; tile += cstride) {
-        ++seq;
-        const bool dbg = kp.dbg != nullptr && blockIdx.x == 0 && seq < 64;
-        if (dbg && lane == 0) kp.dbg[(1 * 64 + seq) * 4 + 0] = clock64();
-        mbar_wait(&tail->tmem_empty[acc], acc_ph ^ 1);
-        tc_fence_after();
-        if (dbg && lane == 0) kp.dbg[(1 * 64 + seq) * 4 + 1] = clock64();
-        const uint32_t d0 = tm_base + (uint32_t)(acc * S * kp.acc_cols);
-        long long bwait = 0;
-        for (int cb = 0; cb < kp.kblocks; ++cb) {
-          const long long ta = dbg ? clock64() : 0;
-          mbar_wait(&tail->a_full[ast], aph);
-          tc_fence_after();
-          if (dbg) bwait += clock64() - ta;
-          // Descriptor arithmetic is hoisted: per (channel block, weight stage) one base descriptor each; taps,
-          // sub-tiles and k-steps only add precomputed 16-byte-unit offsets to the low word.
-          const uint64_t a_desc0 = umma_desc_sbo(smem_u32(a_base + (size_t)ast * kp.a_bytes), a_row_bytes, sbo);
-          for (int tg = 0; tg < tap_groups; ++tg) {
-            const long long tb = dbg ? clock64() : 0;
-            mbar_wait(&tail->b_full[bst], kp.b_resident ? 0u : bph);  // resident: filled once, phase 0 stays complete
-            tc_fence_after();
-            if (dbg) bwait += clock64() - tb;
-            const uint64_t b_desc0 = umma_desc_kmajor(smem_u32(b_base + (size_t)bst * kp.b_bytes), row_bytes);
-            for (int ti = 0; ti < G; ++ti) {
-              const int tap = tg * G + ti;
-              const uint64_t bd = b_desc0 + (uint64_t)((uint32_t)ti * tap_b_units);
-              const uint64_t ad = a_desc0 + (uint64_t)(uint32_t)kp.hs_tap_desc[tap];
-              const uint32_t first = (uint32_t)((cb | tap) != 0);
-#pragma unroll
-              for (int j = 0; j < kS; ++j) {
-#pragma unroll
-                for (int k = 0; k < kSteps; ++k) {
-                  const uint32_t accf = k == 0 ? first : 1u;
-                  if (kPair)
-                    umma_f16_2sm_p(d0 + (uint32_t)j * acc_cols, ad + (uint64_t)j * sub_units + (uint64_t)(2 * k),
-                                   bd + (uint64_t)(2 * k), idesc, accf, lead);
-                  else
-                    umma_f16_p(d0 + (uint32_t)j * acc_cols, ad + (uint64_t)j * sub_units + (uint64_t)(2 * k),
-                               bd + (uint64_t)(2 * k), idesc, accf, lead);
-                }
-              }
-            }
-            if (!kp.b_resident) {
-              if (pair) umma_commit_2sm_p(&tail->b_empty[bst], lead); else umma_commit_p(&tail->b_empty[bst], lead);
-            }
-            if (++bst == kp.b_stages) {
-              bst = 0;
-              bph ^= 1;
-            }
-          }
-          if (pair) umma_commit_2sm_p(&tail->a_empty[ast], lead); else umma_commit_p(&tail->a_empty[ast], lead);
-          if (++ast == kp.a_stages) {
-            ast = 0;
-            aph ^= 1;
-          }
-        }
-        if (pair) umma_commit_2sm_p(&tail->tmem_full[acc], lead); else umma_commit_p(&tail->tmem_full[acc], lead);
-        if (dbg && lane == 0) {
-          kp.dbg[(1 * 64 + seq) * 4 + 2] = bwait;  // cycles this tile spent waiting for operands (a_full + b_full)
-          kp.dbg[(1 * 64 + seq) * 4 + 3] = clock64();
-        }
-        if (++acc == kp.acc_stages) {
-          acc = 0;
-          acc_ph ^= 1;
-        }
-      }
-    }
-    __syncwarp();
-  } else {
-    // ===== epilogue: up to three groups of 4 warps (2-5, 7-10, 11-14), tiles round-robin; S sub-tiles of 16 rows x 8 columns each
-    const int egroup = warp >= 7 ? 1 + ((warp - 7) >> 2) : 0;
-    const int quarter = warp & 3;
-    const int m = quarter * 32 + lane;
-    const int row = m >> 3, col = m & 7;
-    const bool fast = kEpi != PB_EPI_GENERIC || epilogue_fast_ok(kp);  // the host picks a plain class only when it holds
-    int seq = egroup, acc = egroup;  // sequence number / accumulator stage / phase by counters (egroups <= acc_stages)
-    uint32_t acc_ph = 0;
-    for (int tile = cta0 + egroup * cstride; egroup < kp.egroups && tile < kp.total_tiles;
-         tile += kp.egroups * cstride, seq += kp.egroups) {
-      const HaloTile t = halo_decode(kp, tile, crank);
-      const bool dbg = kp.dbg != nullptr && blockIdx.x == 0 && seq < 64 && (threadIdx.x == 64 || (threadIdx.x >= 224 && ((threadIdx.x - 224) & 127) == 0));
-      if (dbg) kp.dbg[(2 * 64 + seq) * 4 + 0] = clock64();
-      mbar_wait(&tail->tmem_full[acc], acc_ph);
-      tc_fence_after();
-      if (dbg) kp.dbg[(2 * 64 + seq) * 4 + 1] = clock64();
-      if (fast) {
-        const int oh = t.th * 16 + row, ow0 = t.tw * 8 * S + col;
-        uint32_t vm = 0;
-#pragma unroll
-        for (int j = 0; j < S; ++j) vm |= (uint32_t)((ow0 + 8 * j < kp.Wo) && (oh < kp.Ho)) << j;
-        const size_t pix0 = ((size_t)t.n * kp.Ho + oh) * kp.Wo + ow0;
-        EpiOut eo;
-        eo.mode = kp.out_mode;
-        const size_t esz = eo.mode == PB_OUT_F32_NHWC ? 4 : 2;
-        const size_t pxb = (size_t)kp.out_C * esz;  // bytes per output pixel
-        size_t opix = pix0, sub_out = 8 * pxb;
-        eo.dx = eo.dy = 0;
-        if (eo.mode == PB_OUT_F16_NHWC_UP2) {
-          opix = ((size_t)t.n * (2 * kp.Ho) + 2 * oh) * (2 * kp.Wo) + 2 * ow0;
-          eo.dx = pxb;
-          eo.dy = (size_t)(2 * kp.Wo) * pxb;
-          sub_out = 16 * pxb;
-        }
-        eo.mode2 = kp.out2_mode;
-        eo.dx2 = eo.dy2 = 0;
-        eo.pool_writer = ((row | col) & 1) == 0;
-        char* obase2 = nullptr;
-        size_t sub_out2 = 0;
-        if (eo.mode2 != PB_OUT2_NONE) {
-          const size_t pxb2 = (size_t)kp.out2_C * 2;
-          size_t pix2;
-          if (eo.mode2 == PB_OUT2_UP2) {
-            pix2 = ((size_t)t.n * (2 * kp.Ho) + 2 * oh) * (2 * kp.Wo) + 2 * ow0;
-            eo.dx2 = pxb2;
-            eo.dy2 = (size_t)(2 * kp.Wo) * pxb2;
-            sub_out2 = 16 * pxb2;
-          } else {  // POOL2 (Ho, Wo even): the pooled pixel of the window whose top-left corner this lane holds
-            pix2 = ((size_t)t.n * (kp.Ho >> 1) + (oh >> 1)) * (kp.Wo >> 1) + (ow0 >> 1);
-            sub_out2 = 4 * pxb2;
-          }
-          obase2 = reinterpret_cast<char*>(kp.out2) + pix2 * pxb2 + (size_t)kp.out2_coff * 2;
-        }
-        const uint32_t t0 = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * S * kp.acc_cols);
-        char* obase = reinterpret_cast<char*>(kp.out) + opix * pxb + (size_t)kp.out_coff * esz;
-          epilogue_fast<kEpi>(kp, eo, t0, S, (uint32_t)kp.acc_cols, (kp.cout_store + 15) >> 4, kp.cout_store, tail->bias,
-                        obase, kp.res + pix0 * kp.res_C + kp.res_coff, sub_out, (size_t)8 * kp.res_C, vm, obase2,
-                        sub_out2);
-      } else if constexpr (kEpi == PB_EPI_GENERIC)
-      for (int j = 0; j < S; ++j) {
-        EpiPix px;
-        px.n = t.n;
-        px.oh = t.th * 16 + row;
-        px.ow = t.tw * 8 * S + 8 * j + col;
-        px.valid = (px.ow < kp.Wo) && (px.oh < kp.Ho);
-        px.pix = ((size_t)px.n * kp.Ho + px.oh) * kp.Wo + px.ow;
-        const uint32_t t_addr =
-            tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)((acc * S + j) * kp.acc_cols);
-        float hacc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-        for (int c = 0; c < kp.BN; c += 32) {
-          uint32_t r0[16], r1[16];
-          const bool second = (c + 16 < kp.BN);
-          tmem_ld16(t_addr + (uint32_t)c, r0);
-          if (second) tmem_ld16(t_addr + (uint32_t)(c + 16), r1);
-          tmem_ld_wait();
-          if (px.valid && c < kp.cout_store) {
-            float v[16];
-            bias_act16(r0, tail->bias + c, kp.act, v,
-                       (kp.res && kp.res_first) ? kp.res + px.pix * kp.res_C + kp.res_coff + c : nullptr);
-            epilogue_store16(kp, px, c, c, v, hacc);
-          }
-          if (second && px.valid && c + 16 < kp.cout_store) {
-            float v[16];
-            bias_act16(r1, tail->bias + c + 16, kp.act, v,
-                       (kp.res && kp.res_first) ? kp.res + px.pix * kp.res_C + kp.res_coff + c + 16 : nullptr);
-            epilogue_store16(kp, px, c + 16, c + 16, v, hacc);
-          }
-        }
-        if (kp.head_n > 0 && px.valid) {
-          const size_t plane = (size_t)kp.Ho * kp.Wo;
-          float* ho = kp.head_out + (size_t)px.n * kp.head_n * plane + (size_t)px.oh * kp.Wo + px.ow;
-#pragma unroll
-          for (int q = 0; q < 8; ++q)
-            if (q < kp.head_n) ho[(size_t)q * plane] = __fdividef(1.f, 1.f + __expf(-(hacc[q] + __ldg(kp.head_b + q))));
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (pair) mbar_arrive_cluster(&tail->tmem_empty[acc], 0);  // the leader's MMA thread waits for both CTAs
-        else mbar_arrive(&tail->tmem_empty[acc]);
-      }
-      if (dbg) kp.dbg[(2 * 64 + seq) * 4 + 2] = clock64();
-      acc += kp.egroups;
-      if (acc >= kp.acc_stages) {
-        acc -= kp.acc_stages;
-        acc_ph ^= 1u;
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (gdbg) gslot[2] = (long long)globaltimer_ns();
-  if (pair) cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after();
-    if (pair) tmem_dealloc2(tmem_base, (uint32_t)kp.tmem_cols);
-    else tmem_dealloc(tmem_base, (uint32_t)kp.tmem_cols);
+  // ===================== consumers: wgmma + epilogue =====================
+  // A sub-tile is 16 image rows x 8 columns = 128 pixels (row m = 8 * image row + column); warpgroup g computes its
+  // image rows 8g .. 8g + 7, i.e. the 8-row groups 8g .. 8g + 7 of every tap's A descriptor.
+  warpgroup_reg_alloc<kConvConsumerRegs>();
+  const int cw = warp - 4, g = cw >> 2, wq = cw & 3;
+  float* scr = tail->scratch + cw * kEpiScratchFloats;
+  const uint32_t sbo = (uint32_t)kp.hs_sbo_rows * a_row_bytes;
+  const uint64_t g_units = (uint64_t)((8u * (uint32_t)g * sbo) >> 4);
+  const uint32_t tap_b_units = ((uint32_t)kp.BN * row_bytes) >> 4;             // 16-byte units
+  const uint64_t sub_units = (uint64_t)((8u * a_row_bytes) >> 4);              // next sub-tile: +8 pixels
+  const int m = 64 * g + 16 * wq + (lane & 15);  // this lane's pixel of each sub-tile in the epilogue
+  const int row = m >> 3, col = m & 7;
+  float acc[kConvAccRegs];
+#pragma unroll
+  for (int i = 0; i < kConvAccRegs; ++i) acc[i] = 0.f;
+  int ast = 0, bst = 0;
+  uint32_t aph = 0, bph = 0;
+  for (int tile = blockIdx.x; tile < kp.total_tiles; tile += gridDim.x) {
+    const HaloTile t = halo_decode(kp, tile);
+    for (int cb = 0; cb < kp.kblocks; ++cb) {
+      mbar_wait(&tail->a_full[ast], aph);
+      // Descriptor arithmetic is hoisted: per (channel block, weight stage) one base descriptor each; taps,
+      // sub-tiles and k-steps only add precomputed 16-byte-unit offsets to the low word.
+      const uint64_t a_desc0 = wgmma_desc(smem_u32(a_base + (size_t)ast * kp.a_bytes), a_row_bytes, sbo) + g_units;
+      for (int tg = 0; tg < tap_groups; ++tg) {
+        mbar_wait(&tail->b_full[bst], kp.b_resident ? 0u : bph);  // resident: filled once, phase 0 stays complete
+        const uint64_t b_desc0 = wgmma_desc_kmajor(smem_u32(b_base + (size_t)bst * kp.b_bytes), row_bytes);
+        wgmma_fence();
+        for (int ti = 0; ti < G; ++ti) {
+          const int tap = tg * G + ti;
+          mma_group<kS, kSteps>(kp.BN, acc, a_desc0 + (uint64_t)(uint32_t)kp.hs_tap_desc[tap], sub_units,
+                                b_desc0 + (uint64_t)((uint32_t)ti * tap_b_units), (uint32_t)((cb | tap) != 0));
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        if (!kp.b_resident) consumer_release(&tail->b_empty[bst], lane);
+        if (++bst == kp.b_stages) {
+          bst = 0;
+          bph ^= 1;
+        }
+      }
+      consumer_release(&tail->a_empty[ast], lane);
+      if (++ast == kp.a_stages) {
+        ast = 0;
+        aph ^= 1;
+      }
+    }
+    wgmma_fence_operands(acc);
+    const int oh = t.th * 16 + row, ow0 = t.tw * 8 * S + col;
+    epilogue_tile<kEpi>(kp, acc, S, 0, tail->bias, scr, lane, [&](int j, bool& pool_writer) {
+      EpiPix px;
+      px.n = t.n;
+      px.oh = oh;
+      px.ow = ow0 + 8 * j;
+      px.valid = (px.ow < kp.Wo) && (px.oh < kp.Ho);
+      px.pix = ((size_t)px.n * kp.Ho + px.oh) * kp.Wo + px.ow;
+      pool_writer = ((row | col) & 1) == 0;
+      return px;
+    });
   }
 }
 
@@ -404,44 +196,18 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 // returns -1 (no error) when the layer should use the per-tap kernel.
 // ------------------------------------------------------------------------------------------------------------
 
-// Final launch configuration shared by the halo and stem set-ups: two CTAs per SM when the tile fits in half an SM's
-// shared memory and 256 TMEM columns (light n-scale YOLO layers), else one CTA per SM with up to three epilogue groups.
+// Launch configuration shared by the halo set-ups: one persistent CTA per SM.
 static void halo_finish_config(ConvPlan* plan) {
-  ConvKParams& kp = plan->kp;
-  const size_t need = (size_t)kp.a_stages * kp.a_bytes + (size_t)kp.b_stages * kp.b_bytes + sizeof(HaloSmemTail) + 1024;
-  const int occ_mode = conv_occ_mode();
-  const int set_cols = kp.hs_S * kp.acc_cols;
-  // Half-SM footprint (224 threads, <= 110 KB, 256 TMEM columns): (a) light layers with many tiles run two CTAs of the
-  // SAME kernel per SM; (b) tiny layers (at most two tiles per SM) take it so that CTAs of CONSECUTIVE kernels can be
-  // co-resident -- with programmatic dependent launch the successor then sits through its launch latency (~10 us from
-  // trigger to release, profiles/r02_chain_timeline.txt) while this kernel still computes.
-  const bool tiny = kp.total_tiles <= 2 * num_sms();
-  const bool occ2 = !kp.pair && occ_mode != 0 && need <= 110 * 1024 &&
-                    ((set_cols * 2 <= 256 && kp.total_tiles > num_sms()) || (occ_mode == 2 && tiny && set_cols <= 256));
-  plan->smem_bytes = need;
-  if (occ2) {
-    if (kp.acc_stages * set_cols > 256) kp.acc_stages = 256 / set_cols;
-    kp.tmem_cols = 256;
-    kp.egroups = 1;
-    plan->threads = 224;
-    plan->grid = kp.total_tiles < 2 * num_sms() ? kp.total_tiles : 2 * num_sms();
-  } else {
-    if (plan->smem_bytes < 120 * 1024) plan->smem_bytes = 120 * 1024;
-    kp.tmem_cols = 512;
-    kp.egroups = kp.pair ? 2 : conv_pick_egroups(kp.acc_stages);
-    plan->threads = conv_threads_for(kp.egroups);
-    plan->grid = kp.total_tiles < num_sms() ? kp.total_tiles : num_sms();
-    if (kp.pair) {  // total_tiles counts pair tiles: two CTAs each
-      const int pairs = kp.total_tiles < num_sms() / 2 ? kp.total_tiles : num_sms() / 2;
-      plan->grid = 2 * pairs;
-    }
-  }
+  const ConvKParams& kp = plan->kp;
+  plan->smem_bytes = (size_t)kp.a_stages * kp.a_bytes + (size_t)kp.b_stages * kp.b_bytes + sizeof(HaloSmemTail) + 1024;
+  plan->threads = kConvThreads;
+  plan->grid = kp.total_tiles < num_sms() ? kp.total_tiles : num_sms();
 }
 
 // Stem (PB_IN_STEM4): 3x3 stride-2 conv over the padded 4-channel input. One TMA box of overlapping 16-element rows
 // (4 pixels x 4 channels, consecutive rows 2 pixels apart) holds, for a tile of 16 x 8S outputs, the three filter
 // rows r = 0..2 as [oh][r][ow] rows of 32 bytes; filter row r of sub-tile j starts at row (r*8S + 8j), 8-row groups
-// (consecutive oh) are 3*8S rows apart.  K = 16 per filter row (12 real), 3 UMMAs per sub-tile.
+// (consecutive oh) are 3*8S rows apart.  K = 16 per filter row (12 real), 3 wgmmas per sub-tile.
 int conv_stem_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode) {
   PB_CHECK(d->ksize == 3 && d->stride == 2 && d->C == 4 && d->cin == 16 && d->c_in_off == 0,
            "conv(stem): needs ksize 3, stride 2, C = 4, cin = 16");
@@ -450,7 +216,7 @@ int conv_stem_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode)
   const int BN = d->cout_pad;
   const int acc_cols = (BN + 31) / 32 * 32;
   int S = 4;
-  while (S > 1 && (S * acc_cols * 2 > 512)) S >>= 1;
+  while (S > 1 && S * acc_cols > 2 * kConvAccRegs) S >>= 1;  // accumulators of S sub-tiles fit the registers
   kp.KB = 16;
   kp.kblocks = 1;
   kp.taps = 3;
@@ -468,7 +234,7 @@ int conv_stem_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode)
   kp.halo_bytes = 16u * 3u * (uint32_t)(8 * S) * 32u;
   kp.hs_a_row_bytes = 32u;
   // Raw-pixel operand (default; PADEL_B200_STEM_RAW=0 selects the overlapping-row box above): the tile's input region --
-  // 34 rows x (16 S + 2) pixels of 8 bytes, every byte once -- is one dense TMA box, and the UMMA descriptor reads the
+  // 34 rows x (16 S + 2) pixels of 8 bytes, every byte once -- is one dense TMA box, and the wgmma descriptor reads the
   // im2col rows out of it: output pixel ow's K = 16 row (pixels 2ow .. 2ow+3) starts 16 bytes after its neighbour's, so
   // in the un-swizzled K-major layout (16-byte rows at a 16-byte pitch, second half of a row LBO = 16 bytes on) the
   // overlapping rows ARE the canonical core matrix; the next output row is two image rows further (SBO), filter row r
@@ -491,10 +257,6 @@ int conv_stem_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode)
   kp.a_stages = 4;
   kp.b_stages = 1;  // the three filter rows are one small box: resident
   kp.b_resident = 1;
-  kp.acc_cols = acc_cols;
-  kp.acc_stages = 512 / (S * acc_cols);
-  if (kp.acc_stages > kConvMaxAcc) kp.acc_stages = kConvMaxAcc;
-  kp.idesc = umma_idesc_f16(BN, 0);
   kp.tiles_w = (kp.Wo + 8 * S - 1) / (8 * S);
   kp.tiles_h = (kp.Ho + 15) / 16;
   kp.tiles_n = kp.N;
@@ -539,7 +301,7 @@ int conv_stem_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode)
 
 int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode) {
   if (d->ksize != 3 || d->stride != 1 || d->cout_pad > 256) return -1;
-  ConvKParams& kp = plan->kp;  // common fields (epilogue, KB, kblocks, idesc, ...) already filled by the caller
+  ConvKParams& kp = plan->kp;  // common fields (epilogue, KB, kblocks, ...) already filled by the caller
   const int BN = d->cout_pad;
   const uint32_t row_bytes = (uint32_t)kp.KB * 2u;
   const int acc_cols = (BN + 31) / 32 * 32;
@@ -561,7 +323,7 @@ int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode)
   for (int pass = resident ? 0 : 1; pass < 2 && bestS == 0; ++pass) {
     resident = resident && pass == 0;
     for (int S = 4; S >= 1; S >>= 1) {
-      if (S * acc_cols * 2 > 512) continue;  // keep >= 2 accumulator sets in TMEM
+      if (S * acc_cols > 2 * kConvAccRegs) continue;  // accumulators of S sub-tiles fit the registers
       const uint32_t halo = 18u * (uint32_t)(8 * S + 2) * row_bytes;
       const uint32_t a_alloc = (halo + 1023u) & ~1023u;
       int g_fit = 0;
@@ -590,25 +352,6 @@ int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode)
   const uint32_t b_alloc = ((uint32_t)G * tap_bytes + 1023u) & ~1023u;
   if (bestS == 0) return -1;
   const int S = bestS, P = 8 * S + 2;
-  // CTA-pair mode (cta_group::2): one M=256 UMMA per instruction slot, each CTA of the pair fetching half of the
-  // weights.  Measured on TrackNet at batch 32 (profiles/r01_layers.txt): the deep-K narrow layers gain (192->64:
-  // 935 -> 757 us = 1.38 PFLOP/s, above the ~1.27 PFLOP/s a single CTA can issue at N = 64; 384->128: 768 -> 676 us;
-  // 128->128: 269 -> 231 us), shallow-K layers (cin <= 64) and the 2x2-replicating stores lose a few percent.
-  // Default rule: cin >= 128, plain fp16 store, enough tiles to fill the machine with pairs.
-  // PADEL_B200_CONV_PAIR=0/1 forces it off / on wherever it applies.
-  {
-    const char* ep = getenv("PADEL_B200_CONV_PAIR");
-    const int pm = ep ? atoi(ep) : 2;
-    const bool can = BN % 32 == 0 && BN >= 32 && kp.Ho >= 32;
-    const long pair_tiles = (long)((d->W + 8 * S - 1) / (8 * S)) * ((kp.Ho + 31) / 32) * kp.N;
-    const bool want = d->cin >= 128 && d->out_mode == PB_OUT_F16_NHWC && pair_tiles >= 2L * (num_sms() / 2);
-    kp.pair = (can && (pm == 1 || (pm == 2 && want))) ? 1 : 0;
-    if (kp.pair && resident) {  // forced pair mode: stream the weights (each CTA holds half of them)
-      resident = false;
-      if (G == 9 && (size_t)2 * (((18u * (uint32_t)(8 * bestS + 2) * row_bytes) + 1023u) & ~1023u) + (size_t)2 * b_alloc > budget)
-        return -1;
-    }
-  }
   kp.b_resident = resident ? 1 : 0;
   kp.hs_S = S;
   kp.hs_P = P;
@@ -627,46 +370,30 @@ int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode)
   kp.halo_bytes = 18u * (uint32_t)P * row_bytes;
   kp.hs_a_row_bytes = row_bytes;
   kp.a_bytes = (kp.halo_bytes + 1023u) & ~1023u;
-  kp.b_tx_bytes = (uint32_t)G * tap_bytes / (kp.pair ? 2u : 1u);  // per CTA
+  kp.b_tx_bytes = (uint32_t)G * tap_bytes;
   kp.b_bytes = b_alloc;
   kp.a_stages = 2;
   if (resident) {
     // the filter bank occupies kblocks fixed slots; whatever is left goes to halo buffers (up to kHaloMaxA)
     kp.b_stages = kp.kblocks;
-    const bool tiny_mode = conv_occ_mode() == 2 && !kp.pair &&
-                           (long)((kp.Wo + 8 * S - 1) / (8 * S)) * ((kp.Ho + 15) / 16) * kp.N <= 2L * num_sms();
-    const bool small = (size_t)2 * kp.a_bytes + res_total + sizeof(HaloSmemTail) + 1024 <= 108 * 1024 &&
-                       (S * acc_cols * 2 <= 256 || (tiny_mode && S * acc_cols <= 256));
-    const size_t budget2 = small ? (size_t)108 * 1024 - sizeof(HaloSmemTail) - 1024 : budget;
-    int as = (int)((budget2 - res_total) / kp.a_bytes);
+    int as = (int)((budget - res_total) / kp.a_bytes);
     if (as > kHaloMaxA) as = kHaloMaxA;
     if (as > 2 * kp.kblocks + 1) as = 2 * kp.kblocks + 1;
     kp.a_stages = as < 2 ? 2 : as;
   } else {
-  // light layers: size the rings for half an SM so that two CTAs can be co-resident (see halo_finish_config)
-  const int min_b_small = G == 9 ? 2 : (G == 3 ? 3 : 4);
-  const bool tiny_mode = conv_occ_mode() == 2 && !kp.pair &&
-                         (long)((kp.Wo + 8 * S - 1) / (8 * S)) * ((kp.Ho + 15) / 16) * kp.N <= 2L * num_sms();
-  const bool small = (size_t)2 * kp.a_bytes + (size_t)min_b_small * b_alloc + sizeof(HaloSmemTail) + 1024 <= 108 * 1024 &&
-                     (S * acc_cols * 2 <= 256 || (tiny_mode && S * acc_cols <= 256));
-  const size_t budget2 = small ? (size_t)108 * 1024 - sizeof(HaloSmemTail) - 1024 : budget;
-  size_t rest = budget2 - (size_t)2 * kp.a_bytes;
-  if (kp.kblocks > 2 && rest > (size_t)kp.a_bytes + 4 * (size_t)b_alloc) {  // a third halo buffer when K is deep
-    kp.a_stages = 3;
-    rest -= kp.a_bytes;
+    size_t rest = budget - (size_t)2 * kp.a_bytes;
+    if (kp.kblocks > 2 && rest > (size_t)kp.a_bytes + 4 * (size_t)b_alloc) {  // a third halo buffer when K is deep
+      kp.a_stages = 3;
+      rest -= kp.a_bytes;
+    }
+    int bs = (int)(rest / b_alloc);
+    if (bs > kHaloMaxB) bs = kHaloMaxB;
+    if (bs > 9 * kp.kblocks / G * 2) bs = 9 * kp.kblocks / G * 2;
+    if (bs < 2) bs = 2;
+    kp.b_stages = bs;
   }
-  int bs = (int)(rest / b_alloc);
-  if (bs > kHaloMaxB) bs = kHaloMaxB;
-  if (bs > 9 * kp.kblocks / G * 2) bs = 9 * kp.kblocks / G * 2;
-  if (bs < 2) bs = 2;
-  kp.b_stages = bs;
-  }
-  kp.acc_cols = acc_cols;
-  kp.acc_stages = 512 / (S * acc_cols);
-  if (kp.acc_stages > kConvMaxAcc) kp.acc_stages = kConvMaxAcc;
-  kp.idesc = kp.pair ? umma_idesc_f16_m256(BN) : umma_idesc_f16(BN, 0);
   kp.tiles_w = (kp.Wo + 8 * S - 1) / (8 * S);
-  kp.tiles_h = kp.pair ? (kp.Ho + 31) / 32 : (kp.Ho + 15) / 16;
+  kp.tiles_h = (kp.Ho + 15) / 16;
   kp.tiles_n = kp.N;
   kp.total_tiles = kp.tiles_w * kp.tiles_h * kp.tiles_n;
   halo_finish_config(plan);
@@ -689,7 +416,7 @@ int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode)
   {
     cuuint64_t dims[3] = {(cuuint64_t)d->cin, (cuuint64_t)d->cout_pad, 9};
     cuuint64_t strides[2] = {(cuuint64_t)d->cin * 2, (cuuint64_t)d->cin * d->cout_pad * 2};
-    cuuint32_t box[3] = {(cuuint32_t)kp.KB, (cuuint32_t)(kp.pair ? BN / 2 : BN), (cuuint32_t)G};
+    cuuint32_t box[3] = {(cuuint32_t)kp.KB, (cuuint32_t)BN, (cuuint32_t)G};
     cuuint32_t estr[3] = {1, 1, 1};
     CUresult r = encode(&plan->tmap_w, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(d->weight), dims,
                         strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -703,9 +430,8 @@ int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode)
 // pixels, S accumulator sets) instead of the per-tap kernel's 128, and the whole filter bank (cin x cout, one box per
 // channel block) is fetched ONCE per CTA and stays in shared memory -- the per-tap kernel re-reads it from L2 for every
 // 128-pixel tile, as many bytes as the activations when cin ~ cout, and pays its fixed per-tile costs four times as
-// often.  Measured on the pose program (batch 32, profiles/r02_layers_final.txt): cin 32 -> 32 @320^2 152 -> 93 us; every
-// layer with cin >= 64 is 0-15 % SLOWER than on the per-tap kernel (whose flattened 128-pixel tiles waste nothing at the
-// image edges and whose K loop is deeper).  Default rule therefore: cin <= 32; PADEL_B200_CONV_HALO1=0 disables it, =2
+// often.  That pays off for the narrow layers of the pose program (cin 32 -> 32 @320^2); wider layers stay on the
+// per-tap kernel, whose flattened 128-pixel tiles waste nothing at the image edges and whose K loop is deeper.  Default rule therefore: cin <= 32; PADEL_B200_CONV_HALO1=0 disables it, =2
 // takes every 1x1 layer whose bank fits next to two activation buffers.
 int conv_halo_1x1_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode) {
   static const int enabled = [] {
@@ -727,7 +453,7 @@ int conv_halo_1x1_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn enc
   if (kp.kblocks > kHaloMaxB || res_total > 120 * 1024) return -1;
   int S = 0;
   for (int s = 4; s >= 1; s >>= 1) {
-    if (s * acc_cols * 2 > 512) continue;  // keep >= 2 accumulator sets in TMEM
+    if (s * acc_cols > 2 * kConvAccRegs) continue;  // accumulators of S sub-tiles fit the registers
     const uint32_t a_alloc = (16u * (uint32_t)(8 * s) * row_bytes + 1023u) & ~1023u;
     if ((size_t)2 * a_alloc + res_total > budget) continue;
     if (s > 1 && d->W <= 8 * (s / 2)) continue;  // a narrower tile already covers the row
@@ -736,7 +462,6 @@ int conv_halo_1x1_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn enc
   }
   if (S == 0) return -1;
   const int P = 8 * S;
-  kp.pair = 0;
   kp.b_resident = 1;
   kp.hs_S = S;
   kp.hs_P = P;
@@ -756,17 +481,11 @@ int conv_halo_1x1_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn enc
   kp.b_bytes = res_box;
   kp.b_stages = kp.kblocks;
   {
-    const bool small = (size_t)2 * kp.a_bytes + res_total + sizeof(HaloSmemTail) + 1024 <= 108 * 1024 && S * acc_cols * 2 <= 256;
-    const size_t budget2 = small ? (size_t)108 * 1024 - sizeof(HaloSmemTail) - 1024 : budget;
-    int as = (int)((budget2 - res_total) / kp.a_bytes);
+    int as = (int)((budget - res_total) / kp.a_bytes);
     if (as > kHaloMaxA) as = kHaloMaxA;
     if (as > 2 * kp.kblocks + 1) as = 2 * kp.kblocks + 1;
     kp.a_stages = as < 2 ? 2 : as;
   }
-  kp.acc_cols = acc_cols;
-  kp.acc_stages = 512 / (S * acc_cols);
-  if (kp.acc_stages > kConvMaxAcc) kp.acc_stages = kConvMaxAcc;
-  kp.idesc = umma_idesc_f16(BN, 0);
   kp.tiles_w = (kp.Wo + 8 * S - 1) / (8 * S);
   kp.tiles_h = (kp.Ho + 15) / 16;
   kp.tiles_n = kp.N;
@@ -824,7 +543,7 @@ int conv_halo_s2_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn enco
   const size_t budget = 196 * 1024;
   int S = 0;
   for (int s = 4; s >= 1; s >>= 1) {
-    if (s * acc_cols * 2 > 512) continue;
+    if (s * acc_cols > 2 * kConvAccRegs) continue;
     const uint32_t halo = 34u * (uint32_t)(8 * s + 1) * a_row;
     if ((size_t)2 * ((halo + 1023u) & ~1023u) + (size_t)2 * b_alloc <= budget) {
       S = s;
@@ -833,7 +552,6 @@ int conv_halo_s2_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn enco
   }
   if (S == 0) return -1;
   const int P = 8 * S + 1;
-  kp.pair = 0;
   kp.KB = d->cin;
   kp.kblocks = 1;
   kp.hs_S = S;
@@ -860,10 +578,6 @@ int conv_halo_s2_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn enco
   kp.a_stages = 2;
   kp.b_stages = 1;  // all nine taps are one box: resident
   kp.b_resident = 1;
-  kp.acc_cols = acc_cols;
-  kp.acc_stages = 512 / (S * acc_cols);
-  if (kp.acc_stages > kConvMaxAcc) kp.acc_stages = kConvMaxAcc;
-  kp.idesc = umma_idesc_f16(BN, 0);
   kp.tiles_w = (kp.Wo + 8 * S - 1) / (8 * S);
   kp.tiles_h = (kp.Ho + 15) / 16;
   kp.tiles_n = kp.N;
@@ -898,10 +612,10 @@ int conv_halo_s2_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn enco
 
 typedef void (*HaloKernelFn)(CUtensorMap, CUtensorMap, ConvKParams);
 
-template <bool kPair, int kEpi>
+template <int kEpi>
 static HaloKernelFn halo_kernel_for(int S, int steps) {
 #define PB_HALO_CASE(s_, k_) \
-  if (S == s_ && steps == k_) return conv_halo_kernel<kPair, s_, k_, kEpi>;
+  if (S == s_ && steps == k_) return conv_halo_kernel<s_, k_, kEpi>;
   PB_HALO_CASE(1, 1) PB_HALO_CASE(1, 2) PB_HALO_CASE(1, 4)
   PB_HALO_CASE(2, 1) PB_HALO_CASE(2, 2) PB_HALO_CASE(2, 4)
   PB_HALO_CASE(4, 1) PB_HALO_CASE(4, 2) PB_HALO_CASE(4, 4)
@@ -909,15 +623,13 @@ static HaloKernelFn halo_kernel_for(int S, int steps) {
   return nullptr;
 }
 
-// CTA-pair layers are deep (cin >= 128) and tensor-bound: the run-time epilogue only
 static HaloKernelFn halo_kernel_pick(const ConvPlan* plan) {
   const ConvKParams& kp = plan->kp;
   const int S = kp.hs_S, steps = kp.KB / 16;
-  if (kp.pair) return halo_kernel_for<true, PB_EPI_GENERIC>(S, steps);
-  if (plan->epi == PB_EPI_SILU) return halo_kernel_for<false, PB_EPI_SILU>(S, steps);
-  if (plan->epi == PB_EPI_RELU) return halo_kernel_for<false, PB_EPI_RELU>(S, steps);
-  if (plan->epi == PB_EPI_SILU_RES) return halo_kernel_for<false, PB_EPI_SILU_RES>(S, steps);
-  return halo_kernel_for<false, PB_EPI_GENERIC>(S, steps);
+  if (plan->epi == PB_EPI_SILU) return halo_kernel_for<PB_EPI_SILU>(S, steps);
+  if (plan->epi == PB_EPI_RELU) return halo_kernel_for<PB_EPI_RELU>(S, steps);
+  if (plan->epi == PB_EPI_SILU_RES) return halo_kernel_for<PB_EPI_SILU_RES>(S, steps);
+  return halo_kernel_for<PB_EPI_GENERIC>(S, steps);
 }
 
 int conv_halo_launch(const ConvPlan* plan, cudaStream_t stream) {
@@ -925,13 +637,10 @@ int conv_halo_launch(const ConvPlan* plan, cudaStream_t stream) {
   HaloKernelFn fn = halo_kernel_pick(plan);
   PB_CHECK(fn != nullptr, "conv(halo): no kernel instantiation for S=%d, k-steps=%d", kp.hs_S, kp.KB / 16);
   PB_CUDA((cudaError_t)ensure_dynamic_smem(reinterpret_cast<const void*>(fn), 227 * 1024));
-  cudaError_t le = launch_ex(fn, dim3(plan->grid), dim3(plan->threads), plan->smem_bytes, stream, kp.pair ? 2 : 1,
-                              plan->pdl != 0,
-                              plan->tmap_a, plan->tmap_w, plan->kp);
-  PB_CHECK(le == cudaSuccess,
-           "conv(halo): launch failed: %s (pair %d, grid %d, threads %d, smem %zu, tiles %d, S %d, BN %d, KB %d)",
-           cudaGetErrorString(le), kp.pair, plan->grid, plan->threads, plan->smem_bytes, kp.total_tiles, kp.hs_S, kp.BN,
-           kp.KB);
+  cudaError_t le = launch_ex(fn, dim3(plan->grid), dim3(plan->threads), plan->smem_bytes, stream, 1, plan->pdl != 0,
+                             plan->tmap_a, plan->tmap_w, plan->kp);
+  PB_CHECK(le == cudaSuccess, "conv(halo): launch failed: %s (grid %d, threads %d, smem %zu, tiles %d, S %d, BN %d, KB %d)",
+           cudaGetErrorString(le), plan->grid, plan->threads, plan->smem_bytes, kp.total_tiles, kp.hs_S, kp.BN, kp.KB);
   count_launch();
   return 0;
 }

@@ -1,21 +1,18 @@
-// Fused conv(k1|k3, s1|s2) + bias + activation (+ residual) as an implicit GEMM on Blackwell tensor cores.
+// Fused conv(k1|k3, s1|s2) + bias + activation (+ residual) as an implicit GEMM on Hopper tensor cores (wgmma).
 //
 //   D[M = 128 output pixels, N = BN out-channels] += A[M, K] * B[N, K]^T,   K = taps x input channels
 //
 // * A (activations, NHWC fp16) is fetched by TMA in tiled mode: one box = a (TN x TH x TW) patch of pixels x KB
 //   channels, shifted by the filter tap; out-of-bounds coordinates are zero-filled by TMA, which implements the
 //   conv zero padding for free.  Stride-2 convs read a 5-D view (N, H/2, 2, W/2, 2C) of the same tensor so every
-//   tap is again a dense box.  The box lands in shared memory directly in the UMMA K-major swizzled layout
+//   tap is again a dense box.  The box lands in shared memory directly in the wgmma K-major swizzled layout
 //   (one pixel = one KB*2-byte row; swizzle 32/64/128B == row size).
 // * B (weights, fp16 [tap][cout][cin]) is fetched by TMA the same way.
-// * warp 0 = TMA producer (activations), warp 6 = TMA producer (weights), warp 1 = tcgen05.mma issuer (whole warp on
-//   warp-uniform values, elect.sync-predicated instructions), warps 2-5 / 7-10 / 11-14 = up to three epilogue groups
-//   taking tiles round-robin (tcgen05.ld TMEM -> regs -> bias/act/residual -> global).  Up to 8 accumulator sets in
-//   TMEM so the epilogues of tiles i-2..i overlap the MMAs of tile i+1.  Persistent CTAs (one per SM, or two for
-//   light layers), static tile striding, tile coordinates via fast division.
+// * warps 0 / 1 = TMA producers (activations / weights); warpgroups 1-2 = consumers, each issuing the wgmmas of 64
+//   rows (register accumulators) and then storing them.  Persistent CTAs, static tile striding, fast-division decode.
 //
 // Replaces: ultralytics Conv/C2f/Bottleneck/Detect convs (3P, SURVEY App. A.2) and TrackNet Conv2DBlock
-// (/root/reference/trackers/ball_tracker/models.py:5-17) with BN folded into weight/bias.
+// (reference trackers/ball_tracker/models.py:5-17) with BN folded into weight/bias.
 #include <cstdlib>
 #include <cstring>
 #include <mutex>
@@ -26,14 +23,15 @@
 
 namespace pb {
 
+// shared memory for the operand rings: what the 227 KB of an SM leaves beside the tail (bias, barriers, epilogue
+// scratch) and the alignment slack
+constexpr size_t kConvStageBudget = 196 * 1024;
+
 struct ConvSmemTail {
   uint64_t full[kConvMaxStages];
   uint64_t empty[kConvMaxStages];
-  uint64_t tmem_full[kConvMaxAcc];
-  uint64_t tmem_empty[kConvMaxAcc];
-  uint32_t tmem_base;
-  uint32_t pad_[3];
   float bias[kConvMaxCout];  // staged once per CTA
+  float scratch[kConvConsumerWarps * kEpiScratchFloats];  // epilogue transposition, one slice per consumer warp
 };
 
 struct TileCoord {
@@ -49,7 +47,7 @@ __device__ __forceinline__ TileCoord decode_tile(const ConvKParams& kp, int tile
 }
 
 template <int kEpi>
-__global__ void __launch_bounds__(kConvMaxThreads, 1)
+__global__ void __launch_bounds__(kConvThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
                const __grid_constant__ ConvKParams kp) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -60,54 +58,34 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  // bring-up timeline (libpadel_b200_debug.so only: kp.dbg is NULL in the product build): GPU-wide nanosecond stamps of
-  // the first and the last CTA -- entry, after griddepcontrol.wait, exit -- to see how consecutive layers overlap
-  const bool gdbg = kp.dbg != nullptr && threadIdx.x == 0 && (blockIdx.x == 0 || blockIdx.x == gridDim.x - 1);
-  long long* gslot = kp.dbg + (3 * 64 + (blockIdx.x == 0 ? 0 : 1)) * 4;
-  if (gdbg) gslot[0] = (long long)globaltimer_ns();
   const int k_iters = kp.taps * kp.kblocks;
 
-  if (warp == 0 && lane == 0) tma_prefetch_desc(&tmap_a);
-  if (warp == 6 && lane == 0) tma_prefetch_desc(&tmap_w);
-  if (warp == 1 && lane == 0) {
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&tmap_a);
     for (int i = 0; i < kp.stages; ++i) {
       mbar_init(&tail->full[i], 2);  // A producer + B producer (each arrives with its expected bytes)
-      mbar_init(&tail->empty[i], 1);
-    }
-    for (int i = 0; i < kp.acc_stages; ++i) {
-      mbar_init(&tail->tmem_full[i], 1);
-      mbar_init(&tail->tmem_empty[i], 4);  // one arrive per epilogue warp
+      mbar_init(&tail->empty[i], kConvConsumerWarps);
     }
     fence_mbar_init();
   }
-  if (warp == 2) {
-    tmem_alloc(&tail->tmem_base, (uint32_t)kp.tmem_cols);
-    tmem_relinquish();
-  }
+  if (warp == 1 && lane == 0) tma_prefetch_desc(&tmap_w);
   for (int i = threadIdx.x; i < kp.cout_pad; i += blockDim.x) tail->bias[i] = kp.bias[i];
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tail->tmem_base;
   // PDL: the prologue above touched constant data only; from here on activations are read and written.  The weight
-  // producer (warp 6) reads constants only and starts fetching while the previous kernel is still running.
+  // producer (warp 1) reads constants only and starts fetching while the previous kernel is still running.
   griddep_launch_dependents();
-  if (warp != 6) griddep_wait();
-  if (gdbg) gslot[1] = (long long)globaltimer_ns();
+  if (warp != 1) griddep_wait();
 
-  if (warp == 0) {
-    // ============================== TMA producer: activations ==============================
-    if (lane == 0) {
+  if (warp < 4) {
+    warpgroup_reg_dealloc<kConvProducerRegs>();
+    if (warp == 0 && lane == 0) {
+      // ============================== TMA producer: activations ==============================
       int stage = 0;
       uint32_t phase = 0;
       const int TW = 1 << kp.tw_log2, TH = 1 << kp.th_log2;
       const int TN = 128 >> (kp.tw_log2 + kp.th_log2);
-      int seq = -1;
       for (int tile = blockIdx.x; tile < kp.total_tiles; tile += gridDim.x) {
         const TileCoord tc = decode_tile(kp, tile);
-        ++seq;
-        const bool dbg = kp.dbg != nullptr && blockIdx.x == 0 && seq < 64;
-        if (dbg) kp.dbg[(0 * 64 + seq) * 4 + 0] = clock64();
         for (int tap = 0; tap < kp.taps; ++tap) {
           const int cw = tc.tw * TW + kp.tap_dw[tap];
           const int ch = tc.th * TH + kp.tap_dh[tap];
@@ -123,13 +101,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
             }
           }
         }
-        if (dbg) kp.dbg[(0 * 64 + seq) * 4 + 1] = clock64();
       }
-    }
-    __syncwarp();
-  } else if (warp == 6) {
-    // ============================== TMA producer: weights (issued in parallel with warp 0) =================
-    if (lane == 0) {
+    } else if (warp == 1 && lane == 0) {
+      // ============================== TMA producer: weights (issued in parallel with warp 0) =================
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < kp.total_tiles; tile += gridDim.x) {
@@ -149,167 +123,62 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         }
       }
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ============================== UMMA issuer ==============================
-    // All 32 lanes run the loop on warp-uniform values (descriptors stay in uniform registers); only the elected
-    // lane's tcgen05 instructions take effect.
-    {
-      const uint32_t lead = elect_one();
-      const uint32_t tm_base = __shfl_sync(0xffffffffu, tmem_base, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      const uint32_t swz = (uint32_t)kp.KB * 2u;
-      const int ksteps = kp.KB / 16;
-      int seq = -1;
-      for (int tile = blockIdx.x; tile < kp.total_tiles; tile += gridDim.x) {
-        ++seq;
-        const bool dbg = kp.dbg != nullptr && blockIdx.x == 0 && seq < 64 && lane == 0;
-        if (dbg) kp.dbg[(1 * 64 + seq) * 4 + 0] = clock64();
-        mbar_wait(&tail->tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        if (dbg) kp.dbg[(1 * 64 + seq) * 4 + 1] = clock64();
-        const uint32_t d_tmem = tm_base + (uint32_t)(acc * kp.acc_cols);
-        for (int it = 0; it < k_iters; ++it) {
-          mbar_wait(&tail->full[stage], phase);
-          tc_fence_after();
-          if (dbg && it == 0) kp.dbg[(1 * 64 + seq) * 4 + 2] = clock64();
-          const uint32_t a_addr = smem_u32(smem + (size_t)stage * stage_bytes);
-          const uint32_t b_addr = a_addr + kp.a_bytes;
-          const uint64_t adesc = umma_desc_kmajor(a_addr, swz);
-          const uint64_t bdesc = umma_desc_kmajor(b_addr, swz);
-#pragma unroll 4
-          for (int k = 0; k < ksteps; ++k) {
-            // advance 16 K-elements = 32 bytes inside the swizzle row: +2 in the (addr >> 4) field
-            umma_f16_p(d_tmem, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), kp.idesc,
-                       (uint32_t)((it | k) != 0), lead);
-          }
-          umma_commit_p(&tail->empty[stage], lead);  // frees the smem slot when these MMAs retire
-          if (++stage == kp.stages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit_p(&tail->tmem_full[acc], lead);  // accumulator ready for the epilogue
-        if (dbg) kp.dbg[(1 * 64 + seq) * 4 + 3] = clock64();
-        if (++acc == kp.acc_stages) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
-      }
-    }
-    __syncwarp();
-  } else {
-    // ============ epilogue: up to three groups of 4 warps (2-5, 7-10, 11-14), tiles round-robin; one TMEM lane quarter per warp
-    const int egroup = warp >= 7 ? 1 + ((warp - 7) >> 2) : 0;
-    const int quarter = warp & 3;
-    const int p = quarter * 32 + lane;  // row of the M=128 tile handled by this thread
-    const int TWm = (1 << kp.tw_log2) - 1, THm = (1 << kp.th_log2) - 1;
-    const int tw_i = p & TWm;
-    const int th_i = (p >> kp.tw_log2) & THm;
-    const int tn_i = p >> (kp.tw_log2 + kp.th_log2);
-    const bool fast = kEpi != PB_EPI_GENERIC || epilogue_fast_ok(kp);  // the host picks a plain class only when it holds
-    // per-CTA tile sequence number / accumulator stage / phase advance by counters (egroups <= acc_stages)
-    int seq = egroup, acc = egroup;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x + egroup * gridDim.x; egroup < kp.egroups && tile < kp.total_tiles;
-         tile += kp.egroups * gridDim.x, seq += kp.egroups) {
-      const TileCoord tc = decode_tile(kp, tile);
-      EpiPix px;
-      px.ow = (tc.tw << kp.tw_log2) + tw_i;
-      px.oh = (tc.th << kp.th_log2) + th_i;
-      px.n = tc.tn * (128 >> (kp.tw_log2 + kp.th_log2)) + tn_i;
-      px.valid = (px.ow < kp.Wo) && (px.oh < kp.Ho) && (px.n < kp.N);
-      px.pix = ((size_t)px.n * kp.Ho + px.oh) * kp.Wo + px.ow;
-      const bool dbg = kp.dbg != nullptr && blockIdx.x == 0 && seq < 64 && (threadIdx.x == 64 || (threadIdx.x >= 224 && ((threadIdx.x - 224) & 127) == 0));
-      if (dbg) kp.dbg[(2 * 64 + seq) * 4 + 0] = clock64();
-      mbar_wait(&tail->tmem_full[acc], acc_phase);
-      tc_fence_after();
-      if (dbg) kp.dbg[(2 * 64 + seq) * 4 + 1] = clock64();
-      const uint32_t t_addr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * kp.acc_cols);
-      float hacc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};  // fused 1x1 head partial sums
-      const float* sb = tail->bias + tc.nt * kp.BN;
-      if (fast) {
-        int cn = kp.cout_store - tc.nt * kp.BN;  // channels of this N tile that exist
-        cn = cn < kp.BN ? cn : kp.BN;
-        if (cn > 0) {
-          EpiOut eo;
-          eo.mode = kp.out_mode;
-          const size_t esz = eo.mode == PB_OUT_F32_NHWC ? 4 : 2;
-          const size_t pxb = (size_t)kp.out_C * esz;
-          size_t opix = px.pix;
-          eo.dx = eo.dy = 0;
-          if (eo.mode == PB_OUT_F16_NHWC_UP2) {
-            opix = ((size_t)px.n * (2 * kp.Ho) + 2 * px.oh) * (2 * kp.Wo) + 2 * px.ow;
-            eo.dx = pxb;
-            eo.dy = (size_t)(2 * kp.Wo) * pxb;
-          }
-          char* obase = reinterpret_cast<char*>(kp.out) + opix * pxb + (size_t)(kp.out_coff + tc.nt * kp.BN) * esz;
-          const __half* rbase = kp.res + px.pix * kp.res_C + kp.res_coff + tc.nt * kp.BN;
-          eo.mode2 = kp.out2_mode;  // PB_OUT2_NONE | PB_OUT2_UP2 here (pool windows do not map onto this tiling)
-          eo.dx2 = eo.dy2 = 0;
-          eo.pool_writer = false;
-          char* obase2 = nullptr;
-          if (eo.mode2 == PB_OUT2_UP2) {
-            const size_t pxb2 = (size_t)kp.out2_C * 2;
-            const size_t pix2 = ((size_t)px.n * (2 * kp.Ho) + 2 * px.oh) * (2 * kp.Wo) + 2 * px.ow;
-            eo.dx2 = pxb2;
-            eo.dy2 = (size_t)(2 * kp.Wo) * pxb2;
-            obase2 = reinterpret_cast<char*>(kp.out2) + pix2 * pxb2 + (size_t)(kp.out2_coff + tc.nt * kp.BN) * 2;
-          }
-            epilogue_fast<kEpi>(kp, eo, t_addr, 1, 0u, (cn + 15) >> 4, cn, sb, obase, rbase, 0, 0, px.valid ? 1u : 0u,
-                                obase2, 0);
-        }
-      } else if constexpr (kEpi == PB_EPI_GENERIC) {
-      for (int c = 0; c < kp.BN; c += 32) {
-        // two 16-column TMEM loads in flight, one wait
-        uint32_t r0[16], r1[16];
-        const bool second = (c + 16 < kp.BN);
-        tmem_ld16(t_addr + (uint32_t)c, r0);
-        if (second) tmem_ld16(t_addr + (uint32_t)(c + 16), r1);
-        tmem_ld_wait();
-        const int ch0 = tc.nt * kp.BN + c;
-        if (px.valid && ch0 < kp.cout_store) {
-          float v[16];
-          bias_act16(r0, sb + c, kp.act, v,
-                     (kp.res && kp.res_first) ? kp.res + px.pix * kp.res_C + kp.res_coff + ch0 : nullptr);
-          epilogue_store16(kp, px, ch0, c, v, hacc);
-        }
-        if (second && px.valid && ch0 + 16 < kp.cout_store) {
-          float v[16];
-          bias_act16(r1, sb + c + 16, kp.act, v,
-                     (kp.res && kp.res_first) ? kp.res + px.pix * kp.res_C + kp.res_coff + ch0 + 16 : nullptr);
-          epilogue_store16(kp, px, ch0 + 16, c + 16, v, hacc);
-        }
-      }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tail->tmem_empty[acc]);
-      if (dbg) kp.dbg[(2 * 64 + seq) * 4 + 2] = clock64();
-      if (kp.head_n > 0 && px.valid) {
-        const size_t plane = (size_t)kp.Ho * kp.Wo;
-        float* ho = kp.head_out + (size_t)px.n * kp.head_n * plane + (size_t)px.oh * kp.Wo + px.ow;
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          if (j < kp.head_n) ho[(size_t)j * plane] = __fdividef(1.f, 1.f + __expf(-(hacc[j] + __ldg(kp.head_b + j))));
-      }
-      acc += kp.egroups;
-      if (acc >= kp.acc_stages) {
-        acc -= kp.acc_stages;
-        acc_phase ^= 1u;
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (gdbg) gslot[2] = (long long)globaltimer_ns();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, (uint32_t)kp.tmem_cols);
+  // ============================== consumers: wgmma + epilogue ==============================
+  // warpgroup g computes rows 64g .. 64g + 63 of every 128-pixel tile; its warp wq holds rows 64g + 16wq .. +15.
+  warpgroup_reg_alloc<kConvConsumerRegs>();
+  const int cw = warp - 4, g = cw >> 2, wq = cw & 3;
+  float* scr = tail->scratch + cw * kEpiScratchFloats;
+  const uint32_t row_bytes = (uint32_t)kp.KB * 2u;
+  const int ksteps = kp.KB / 16;
+  const int p = 64 * g + 16 * wq + (lane & 15);  // this lane's row of the M = 128 tile in the epilogue
+  const int TWm = (1 << kp.tw_log2) - 1, THm = (1 << kp.th_log2) - 1;
+  const int tw_i = p & TWm;
+  const int th_i = (p >> kp.tw_log2) & THm;
+  const int tn_i = p >> (kp.tw_log2 + kp.th_log2);
+  float acc[kConvAccRegs];
+#pragma unroll
+  for (int i = 0; i < kConvAccRegs; ++i) acc[i] = 0.f;
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < kp.total_tiles; tile += gridDim.x) {
+    const TileCoord tc = decode_tile(kp, tile);
+    int prev = -1;
+    for (int it = 0; it < k_iters; ++it) {
+      mbar_wait(&tail->full[stage], phase);
+      const uint32_t a_addr = smem_u32(smem + (size_t)stage * stage_bytes) + 64u * (uint32_t)g * row_bytes;
+      const uint64_t adesc = wgmma_desc_kmajor(a_addr, row_bytes);
+      const uint64_t bdesc = wgmma_desc_kmajor(smem_u32(smem + (size_t)stage * stage_bytes + kp.a_bytes), row_bytes);
+      wgmma_fence();
+      for (int k = 0; k < ksteps; ++k)  // advance 16 K-elements = 32 bytes inside the swizzle row: +2 in (addr >> 4)
+        mma_group<1, 1>(kp.BN, acc, adesc + (uint64_t)(2 * k), 0, bdesc + (uint64_t)(2 * k), (uint32_t)((it | k) != 0));
+      wgmma_commit();
+      if (prev >= 0) {  // keep one stage of wgmmas in flight; the one before it has retired
+        wgmma_wait<1>();
+        consumer_release(&tail->empty[prev], lane);
+      }
+      prev = stage;
+      if (++stage == kp.stages) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_operands(acc);
+    consumer_release(&tail->empty[prev], lane);
+
+    EpiPix px;
+    px.ow = (tc.tw << kp.tw_log2) + tw_i;
+    px.oh = (tc.th << kp.th_log2) + th_i;
+    px.n = tc.tn * (128 >> (kp.tw_log2 + kp.th_log2)) + tn_i;
+    px.valid = (px.ow < kp.Wo) && (px.oh < kp.Ho) && (px.n < kp.N);
+    px.pix = ((size_t)px.n * kp.Ho + px.oh) * kp.Wo + px.ow;
+    epilogue_tile<kEpi>(kp, acc, 1, tc.nt, tail->bias + tc.nt * kp.BN, scr, lane, [&](int, bool& pool_writer) {
+      pool_writer = false;  // pool windows do not map onto this tiling (halo kernel only)
+      return px;
+    });
   }
 }
 
@@ -335,13 +204,6 @@ static int ilog2(int v) {
   return l;
 }
 
-#ifdef PB_DEBUG_BUILD  // libpadel_b200_debug.so only: clock64 role timelines of CTA 0 (scripts/exp_timeline*.py)
-static long long* g_conv_dbg = nullptr;
-extern "C" void pb_debug_conv_timeline(long long* buf) { g_conv_dbg = buf; }
-#else
-static long long* const g_conv_dbg = nullptr;
-#endif
-
 // Which epilogue instantiation a layer runs: a plain class when the vectorised epilogue applies (the conditions of
 // epilogue_fast_ok) and the layer is activation-only -- no residual, fp16 NHWC store, no secondary output, no fused head.
 // PADEL_B200_CONV_EPI=0 keeps every layer on the run-time epilogue (A/B).
@@ -350,7 +212,7 @@ int conv_epi_class(const pb_conv_desc* d, const ConvKParams& kp) {
     const char* e = getenv("PADEL_B200_CONV_EPI");
     return e ? atoi(e) : 1;
   }();
-  if (!enabled || kp.dbg_flags != 0 || kp.dbg != nullptr) return PB_EPI_GENERIC;
+  if (!enabled || kp.dbg_flags != 0) return PB_EPI_GENERIC;
   if (d->head_n != 0 || d->out2_mode != PB_OUT2_NONE || (reinterpret_cast<uintptr_t>(d->out) & 31) != 0)
     return PB_EPI_GENERIC;
   if (d->out_mode == PB_OUT_F32_NHWC) {  // 32-byte aligned 8-float groups
@@ -447,7 +309,6 @@ static int conv_plan_build_impl(const pb_conv_desc* d, ConvPlan* plan) {
   kp.head_b = d->head_bias;
   kp.head_n = d->head_n;
   kp.head_out = d->head_out;
-  kp.dbg = g_conv_dbg;
   {
     const char* df = getenv("PADEL_B200_CONV_DEBUG");
     kp.dbg_flags = df ? atoi(df) : 0;
@@ -516,42 +377,17 @@ static int conv_plan_build_impl(const pb_conv_desc* d, ConvPlan* plan) {
         kp.tap_d2[t] = (dy != 0) ? 1 : 0;
       }
     }
-  // TMEM accumulator ring: as many buffers as fit (<= 8) so short-K tiles are not bound by the
-  // MMA -> epilogue -> MMA hand-shake latency
-  kp.acc_cols = (kp.BN + 31) / 32 * 32;
-  kp.acc_stages = 512 / kp.acc_cols;
-  if (kp.acc_stages > kConvMaxAcc) kp.acc_stages = kConvMaxAcc;
-  kp.idesc = umma_idesc_f16(kp.BN, 0);
   kp.a_bytes = 128u * kp.KB * 2u;
   kp.b_tx_bytes = (uint32_t)kp.BN * kp.KB * 2u;
   kp.b_bytes = (kp.b_tx_bytes + 1023u) & ~1023u;
   const uint32_t stage_bytes = kp.a_bytes + kp.b_bytes;
-  // Two CTAs per SM for light layers (small stages, narrow N): each gets half the shared memory and 256 TMEM
-  // columns, so one CTA's TMA / epilogue latency is covered by the other's work.  PADEL_B200_CONV_OCC2=0 disables.
-  const int occ_mode = conv_occ_mode();
-  const bool tiny = kp.total_tiles <= 2 * num_sms();  // see halo_finish_config: co-residency of consecutive kernels
-  const bool occ2 = occ_mode != 0 &&
-                    (((size_t)stage_bytes * 6 <= 96 * 1024 && kp.acc_cols * 2 <= 256 && kp.total_tiles > num_sms()) ||
-                     (occ_mode == 2 && tiny && (size_t)stage_bytes * 2 <= 96 * 1024 && kp.acc_cols <= 256));
-  const size_t budget = occ2 ? 96 * 1024 : 200 * 1024;
-  int stages = (int)(budget / stage_bytes);
+  int stages = (int)(kConvStageBudget / stage_bytes);
   if (stages > kConvMaxStages) stages = kConvMaxStages;
   PB_CHECK(stages >= 2, "conv: stage too large (%u bytes)", stage_bytes);
   kp.stages = stages;
   plan->smem_bytes = (size_t)stages * stage_bytes + sizeof(ConvSmemTail) + 1024;
-  if (occ2) {
-    if (kp.acc_stages * kp.acc_cols > 256) kp.acc_stages = 256 / kp.acc_cols;
-    kp.tmem_cols = 256;
-    kp.egroups = 1;
-    plan->threads = 224;
-    plan->grid = kp.total_tiles < 2 * num_sms() ? kp.total_tiles : 2 * num_sms();
-  } else {
-    if (plan->smem_bytes < 120 * 1024) plan->smem_bytes = 120 * 1024;  // force 1 CTA/SM (TMEM: 512 cols)
-    kp.tmem_cols = 512;
-    kp.egroups = conv_pick_egroups(kp.acc_stages);
-    plan->threads = conv_threads_for(kp.egroups);
-    plan->grid = kp.total_tiles < num_sms() ? kp.total_tiles : num_sms();
-  }
+  plan->threads = kConvThreads;
+  plan->grid = kp.total_tiles < num_sms() ? kp.total_tiles : num_sms();
   const CUtensorMapSwizzle swz = kp.KB == 64   ? CU_TENSOR_MAP_SWIZZLE_128B
                                  : kp.KB == 32 ? CU_TENSOR_MAP_SWIZZLE_64B
                                                : CU_TENSOR_MAP_SWIZZLE_32B;
@@ -675,7 +511,7 @@ int conv_reference_launch(const pb_conv_desc* d, cudaStream_t stream) {
   const int Ho = d->H / d->stride, Wo = d->W / d->stride;
   const long total = (long)d->N * Ho * Wo * d->cout_pad;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > (long)num_sms() * 32) blocks = (int)((long)num_sms() * 32);
   conv_reference_kernel<<<blocks, 256, 0, stream>>>(*d, Ho, Wo);
   PB_CUDA(cudaGetLastError());
   count_launch();

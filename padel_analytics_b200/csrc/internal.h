@@ -82,28 +82,12 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 
 // ---- conv plan (built once per layer; holds TMA descriptors + launch geometry) -------------------------------
 constexpr int kConvMaxStages = 12;
-constexpr int kConvMaxAcc = 8;
-// Warp roles of the conv kernels: w0 TMA-A, w1 UMMA issuer, w2-5 epilogue group 0, w6 TMA-B, then 4 warps per further
-// epilogue group (w7-10, w11-14).  Epilogue groups take tiles round-robin; more groups = more warps to hide the
-// dependent-issue latency of the activation math (ncu: the epilogue warps issue ~20% of the time each).  Three groups
-// = 480 threads is the most that keeps 128 registers per thread (19 warps would be capped at 96).
-constexpr int kConvThreads = 352;     // two groups
-constexpr int kConvMaxThreads = 480;  // three groups
-inline int conv_threads_for(int egroups) { return (7 + 4 * (egroups - 1)) * 32; }
-// groups for a 1-CTA-per-SM launch: at most one per accumulator stage (a group may only wait one phase ahead)
-inline int conv_pick_egroups(int acc_stages) {
-  const char* e = getenv("PADEL_B200_CONV_EGROUPS");
-  int want = e ? atoi(e) : 3;
-  if (want < 1 || want > 3) want = 3;
-  if (want > acc_stages) want = acc_stages;
-  return want < 1 ? 1 : want;
-}
-// PADEL_B200_CONV_OCC2: 0 = never two CTAs per SM, 1 = light many-tile layers, 2 (default) = also tiny layers
-inline int conv_occ_mode() {
-  const char* e = getenv("PADEL_B200_CONV_OCC2");
-  const int m = e ? atoi(e) : 1;
-  return m < 0 || m > 2 ? 1 : m;
-}
+// Conv kernels: warpgroup 0 = TMA producers (w0 activations, w1 weights), warpgroups 1-2 = wgmma consumers of 64 rows
+// each; setmaxnreg moves the producers' registers to the consumers' fp32 accumulators (<= 128 per thread).
+constexpr int kConvThreads = 384;
+constexpr int kConvConsumerWarps = 8;
+constexpr int kConvProducerRegs = 40;
+constexpr int kConvConsumerRegs = 232;
 constexpr int kConvMaxCout = 2048;  // ResNet50 layer4 (keypoints_tracker.py:158)
 
 // Division by a launch-time constant as multiply-high + shift (dividend < 2^31): the per-tile coordinate decode of the
@@ -146,12 +130,7 @@ struct ConvKParams {
   int out_C, out_coff, out_mode, cout_store;
   void* out2;  // secondary output (PB_OUT2_*), fast epilogue only
   int out2_C, out2_coff, out2_mode;
-  uint32_t idesc;
   uint32_t a_bytes, b_bytes, b_tx_bytes;
-  int acc_stages, acc_cols;  // TMEM accumulator ring: acc_stages buffers, acc_cols columns apart
-  int tmem_cols;             // TMEM columns allocated by the CTA (power of two; 512 unless two CTAs share an SM)
-  int pair;                  // 1: CTA-pair mode (cluster of 2, cta_group::2 UMMAs issued by the even CTA)
-  int egroups;               // epilogue warp groups (1 with 224 threads / two CTAs per SM, else 2 or 4)
   const float* head_w;
   const float* head_b;
   int head_n;
@@ -164,7 +143,6 @@ struct ConvKParams {
   int hs_tap_off[9];                                   // smem row offset of each tap's first pixel
   int hs_tap_desc[9];                                  // the same in 16-byte descriptor units (offset * row_bytes / 16)
   int dbg_flags;   // PADEL_B200_CONV_DEBUG: bit0 = plain two-MUFU SiLU (default: one reciprocal per four values), bit1 = no fast epilogue
-  long long* dbg;  // optional timeline buffer (CTA 0, first 64 tiles): [role 0..2][64][4] clock64 stamps
 };
 
 struct ConvPlan {

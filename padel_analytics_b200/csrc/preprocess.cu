@@ -116,8 +116,7 @@ pil_horizontal_kernel(const uint8_t* __restrict__ src, int Ws, uint8_t* __restri
 // a thread computes output column xo for R rows with ONE read of its window bounds and filter taps, rows are packed to
 // one 32-bit word per pixel straight from 16-byte global loads (48 bytes = 16 pixels per step, no byte-wise staging),
 // and the R output rows -- contiguous in `tmp` -- leave through shared memory as 16-byte stores.  The one-row kernel
-// above spends ~12 instructions per row and tap (it is instruction-bound: 175 us for 32 x 1080p -> 1280 columns,
-// 5 x its HBM time); this one ~8, and the byte-wise stage / pack / scattered byte stores are gone.
+// above spends ~12 instructions per row and tap (it is instruction-bound, well above its HBM time); this one ~8, and the byte-wise stage / pack / scattered byte stores are gone.
 template <int R>
 __global__ void __launch_bounds__(256)
 pil_horizontal_rows_kernel(const uint8_t* __restrict__ src, int Ws, long rows_total, uint8_t* __restrict__ tmp, int Wo,

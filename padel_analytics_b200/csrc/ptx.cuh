@@ -1,4 +1,4 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (UMMA + TMEM).
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), setmaxnreg, wgmma.
 // Hand-written for this repo; no CUTLASS/CuTe dependency.
 #pragma once
 #include <cstdint>
@@ -50,11 +50,9 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 // ----------------------------------------------------------------------------------------------
 // Programmatic dependent launch (PDL).  A kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization
 // may start while its predecessor in the stream is still running: everything before griddep_wait() (barrier init,
-// TMEM allocation, tensor-map prefetch, bias staging = constant data only) overlaps the predecessor's tail;
+// tensor-map prefetch, bias staging = constant data only) overlaps the predecessor's tail;
 // griddep_wait() returns once the predecessor has completed and its writes are visible.  griddep_launch_dependents()
-// lets the successor's CTAs be scheduled as SMs free up; it is issued only AFTER this CTA owns its TMEM columns, so a
-// successor CTA can never hold TMEM that a CTA of an earlier grid is still waiting for.  Both are no-ops for
-// kernels launched without the attribute.
+// lets the successor's CTAs be scheduled as SMs free up.  Both are no-ops for kernels launched without the attribute.
 // ----------------------------------------------------------------------------------------------
 __device__ __forceinline__ unsigned long long globaltimer_ns() {
   unsigned long long t;
@@ -89,93 +87,16 @@ __device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
-// ----------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, UMMA issue, commit, TMEM loads
-// ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
+// setmaxnreg: producers give registers back, consumers take them (executed by every warp of the warpgroup)
+template <int kRegs>
+__device__ __forceinline__ void warpgroup_reg_dealloc() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs));
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+template <int kRegs>
+__device__ __forceinline__ void warpgroup_reg_alloc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs));
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]; kind::f16 (fp16/bf16 inputs, fp32 accumulate). One thread issues.
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Warp-uniform issue: the whole warp runs the issue loop on warp-uniform values (so the descriptors live in uniform
-// registers and each UMMA costs a couple of uniform adds, instead of a divergent single-lane branch where every
-// tcgen05.mma operand has to be moved to the uniform file through an ELECT / R2UR waterfall), and only the elected
-// lane's instruction takes effect.  `lead` = elect_one() evaluated once.
-__device__ __forceinline__ uint32_t elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(pred));
-  return pred;
-}
-__device__ __forceinline__ void umma_f16_p(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                           uint32_t accumulate, uint32_t lead) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "setp.ne.b32 q, %5, 0;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(lead)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_p(uint64_t* bar, uint32_t lead) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\t"
-      "setp.ne.b32 q, %1, 0;\n\t"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(smem_u32(bar)),
-      "r"(lead)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued UMMAs of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-// TMEM -> registers: this warp's 32 lanes x 16 consecutive fp32 columns (one row per thread).
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
-      "%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// Same wait, but the 16 destination registers of the load are threaded through it ("+r"), so that no use of them can
-// be scheduled before the wait when other work sits between the tcgen05.ld and the wait (software-pipelined epilogue).
-__device__ __forceinline__ void tmem_ld_wait16(uint32_t (&r)[16]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                 "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-               :
-               : "memory");
-}
+
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -187,113 +108,113 @@ __device__ __forceinline__ float rcp_approx(float x) {
   return y;
 }
 
-// UMMA shared-memory matrix descriptor, K-major operand, swizzled canonical layout:
-//   rows of `swz_bytes` (32/64/128) bytes, 8-row groups `8*swz_bytes` apart (SBO), LBO field = 1 (unused).
-//   bits [0,14) addr>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout type.
-__device__ __forceinline__ uint64_t umma_desc_kmajor(uint32_t saddr, uint32_t swz_bytes) {
-  const uint64_t layout = swz_bytes == 128 ? 2ull : (swz_bytes == 64 ? 4ull : 6ull);
-  const uint64_t sbo = (8ull * swz_bytes) >> 4;
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | (1ull << 16) | (sbo << 32) | (1ull << 46) | (layout << 61);
+// wgmma: D[64 x N, regs] (+)= A[64 x 16, smem] * B[N x 16, smem]^T, fp16 in, fp32 out, K-major.  Warp w, lane l:
+// d[4i + 0, 1] = row 16w + l/4, columns 8i + 2(l%4) + {0, 1};  d[4i + 2, 3] = the same columns of row 16w + l/4 + 8.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int kPending>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kPending) : "memory");
 }
-// kind::f16 instruction descriptor: fp32 accumulate, both operands K-major, M=128.
-__host__ __device__ __forceinline__ uint32_t umma_idesc_f16(int n, int is_bf16) {
-  const uint32_t fmt = is_bf16 ? 1u : 0u;
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
-
-
-// ----------------------------------------------------------------------------------------------
-// CTA-pair (cta_group::2) variants: two CTAs of a cluster cooperate on one M=256 UMMA; the even CTA leads.
-// ----------------------------------------------------------------------------------------------
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;  // clears the CTA-parity bit of a shared::cluster address
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t* smem_dst, uint32_t ncols) {  // one warp in EACH CTA of the pair
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish2() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// TMA loads issued by either CTA of the pair; completion bytes are credited to the LEADER's mbarrier
-__device__ __forceinline__ void tma_load_3d_2sm(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                                int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, "
-      "%4, %5}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_5d_2sm(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                                int c2, int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, "
-      "%4, %5, %6, %7}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3),
-      "r"(c4)
-      : "memory");
-}
-// D[tmem, 256 rows over the pair] (+)= A * B : issued by the leader CTA only
-__device__ __forceinline__ void umma_f16_2sm(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_f16_2sm_p(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                               uint32_t accumulate, uint32_t lead) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "setp.ne.b32 q, %5, 0;\n\t"
-      "@q tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(lead)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm_p(uint64_t* bar, uint32_t lead) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\t"
-      "setp.ne.b32 q, %2, 0;\n\t"
-      "@q tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n\t}" ::"r"(
-          smem_u32(bar)),
-      "h"((uint16_t)3), "r"(lead)
-      : "memory");
-}
-// arrive (when the leader's previously issued pair-MMAs retire) on the barrier at this smem offset in BOTH CTAs
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"((uint16_t)3)
-      : "memory");
-}
-// arrive on the barrier at the same smem offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(bar)),
-      "r"(rank)
-      : "memory");
-}
-// kind::f16 instruction descriptor for the pair MMA: M = 256
-__host__ __device__ __forceinline__ uint32_t umma_idesc_f16_m256(int n) {
-  return (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
+// Keeps accumulator reads and writes from moving across an asynchronous wgmma.
+template <int kN>
+__device__ __forceinline__ void wgmma_fence_operands(float (&d)[kN]) {
+#pragma unroll
+  for (int i = 0; i < kN; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
+// Shared-memory matrix descriptor, K-major: addr>>4 | LBO>>4 << 16 | SBO>>4 << 32 | layout << 62 (1/2/3 = 128/64/32-byte
+// swizzle rows of `row_bytes`, 0 = 16-byte un-swizzled rows whose second K half is `lbo_bytes` on); 8-row groups
+// `sbo_bytes` apart.  The swizzle uses absolute address bits: a descriptor may start at any row of an aligned box.
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t saddr, uint32_t row_bytes, uint32_t sbo_bytes,
+                                               uint32_t lbo_bytes = 16) {
+  const uint64_t layout = row_bytes == 128 ? 1ull : (row_bytes == 64 ? 2ull : (row_bytes == 32 ? 3ull : 0ull));
+  return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) |
+         ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | (layout << 62);
+}
+// dense K-major tile (TMA box of rows of `row_bytes`): 8-row groups 8 rows apart
+__device__ __forceinline__ uint64_t wgmma_desc_kmajor(uint32_t saddr, uint32_t row_bytes) {
+  return wgmma_desc(saddr, row_bytes, 8u * row_bytes);
+}
+
+// m64nNk16, N = 16 .. 256 in steps of 16: d[0 .. N/2) of the fragment above.  scale_d = 0 overwrites D.
+template <int kN>
+__device__ __forceinline__ void wgmma_f16(float* d, uint64_t a, uint64_t b, uint32_t scale_d);
+// Operand lists of the specialisations: 8 accumulator registers per macro, RS<k> / DS<k> = the first 8k.
+#define PB_WG_R0 "%0, %1, %2, %3, %4, %5, %6, %7"
+#define PB_WG_R1 "%8, %9, %10, %11, %12, %13, %14, %15"
+#define PB_WG_R2 "%16, %17, %18, %19, %20, %21, %22, %23"
+#define PB_WG_R3 "%24, %25, %26, %27, %28, %29, %30, %31"
+#define PB_WG_R4 "%32, %33, %34, %35, %36, %37, %38, %39"
+#define PB_WG_R5 "%40, %41, %42, %43, %44, %45, %46, %47"
+#define PB_WG_R6 "%48, %49, %50, %51, %52, %53, %54, %55"
+#define PB_WG_R7 "%56, %57, %58, %59, %60, %61, %62, %63"
+#define PB_WG_R8 "%64, %65, %66, %67, %68, %69, %70, %71"
+#define PB_WG_R9 "%72, %73, %74, %75, %76, %77, %78, %79"
+#define PB_WG_R10 "%80, %81, %82, %83, %84, %85, %86, %87"
+#define PB_WG_R11 "%88, %89, %90, %91, %92, %93, %94, %95"
+#define PB_WG_R12 "%96, %97, %98, %99, %100, %101, %102, %103"
+#define PB_WG_R13 "%104, %105, %106, %107, %108, %109, %110, %111"
+#define PB_WG_R14 "%112, %113, %114, %115, %116, %117, %118, %119"
+#define PB_WG_R15 "%120, %121, %122, %123, %124, %125, %126, %127"
+#define PB_WG_D(k) "+f"(d[8 * k]), "+f"(d[8 * k + 1]), "+f"(d[8 * k + 2]), "+f"(d[8 * k + 3]), "+f"(d[8 * k + 4]), \
+      "+f"(d[8 * k + 5]), "+f"(d[8 * k + 6]), "+f"(d[8 * k + 7])
+#define PB_WGMMA(n_, a_, b_, s_, regs_, ops_)                                                              \
+  template <>                                                                                                  \
+  __device__ __forceinline__ void wgmma_f16<n_>(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {          \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" #s_ ", 0;\n\t"                                        \
+                 "wgmma.mma_async.sync.aligned.m64n" #n_ "k16.f32.f16.f16 {" regs_ "}, %" #a_ ", %" #b_             \
+                 ", p, 1, 1, 0, 0;\n\t}"                                                                          \
+                 : ops_                                                                                        \
+                 : "l"(a), "l"(b), "r"(scale_d));                                                              \
+  }
+#define PB_COMMA ,
+#define PB_WG_RS1 PB_WG_R0
+#define PB_WG_RS2 PB_WG_RS1 ", " PB_WG_R1
+#define PB_WG_RS3 PB_WG_RS2 ", " PB_WG_R2
+#define PB_WG_RS4 PB_WG_RS3 ", " PB_WG_R3
+#define PB_WG_RS5 PB_WG_RS4 ", " PB_WG_R4
+#define PB_WG_RS6 PB_WG_RS5 ", " PB_WG_R5
+#define PB_WG_RS7 PB_WG_RS6 ", " PB_WG_R6
+#define PB_WG_RS8 PB_WG_RS7 ", " PB_WG_R7
+#define PB_WG_RS9 PB_WG_RS8 ", " PB_WG_R8
+#define PB_WG_RS10 PB_WG_RS9 ", " PB_WG_R9
+#define PB_WG_RS11 PB_WG_RS10 ", " PB_WG_R10
+#define PB_WG_RS12 PB_WG_RS11 ", " PB_WG_R11
+#define PB_WG_RS13 PB_WG_RS12 ", " PB_WG_R12
+#define PB_WG_RS14 PB_WG_RS13 ", " PB_WG_R13
+#define PB_WG_RS15 PB_WG_RS14 ", " PB_WG_R14
+#define PB_WG_RS16 PB_WG_RS15 ", " PB_WG_R15
+#define PB_WG_DS1 PB_WG_D(0)
+#define PB_WG_DS2 PB_WG_DS1 PB_COMMA PB_WG_D(1)
+#define PB_WG_DS3 PB_WG_DS2 PB_COMMA PB_WG_D(2)
+#define PB_WG_DS4 PB_WG_DS3 PB_COMMA PB_WG_D(3)
+#define PB_WG_DS5 PB_WG_DS4 PB_COMMA PB_WG_D(4)
+#define PB_WG_DS6 PB_WG_DS5 PB_COMMA PB_WG_D(5)
+#define PB_WG_DS7 PB_WG_DS6 PB_COMMA PB_WG_D(6)
+#define PB_WG_DS8 PB_WG_DS7 PB_COMMA PB_WG_D(7)
+#define PB_WG_DS9 PB_WG_DS8 PB_COMMA PB_WG_D(8)
+#define PB_WG_DS10 PB_WG_DS9 PB_COMMA PB_WG_D(9)
+#define PB_WG_DS11 PB_WG_DS10 PB_COMMA PB_WG_D(10)
+#define PB_WG_DS12 PB_WG_DS11 PB_COMMA PB_WG_D(11)
+#define PB_WG_DS13 PB_WG_DS12 PB_COMMA PB_WG_D(12)
+#define PB_WG_DS14 PB_WG_DS13 PB_COMMA PB_WG_D(13)
+#define PB_WG_DS15 PB_WG_DS14 PB_COMMA PB_WG_D(14)
+#define PB_WG_DS16 PB_WG_DS15 PB_COMMA PB_WG_D(15)
+PB_WGMMA(16, 8, 9, 10, PB_WG_RS1, PB_WG_DS1)
+PB_WGMMA(32, 16, 17, 18, PB_WG_RS2, PB_WG_DS2)
+PB_WGMMA(48, 24, 25, 26, PB_WG_RS3, PB_WG_DS3)
+PB_WGMMA(64, 32, 33, 34, PB_WG_RS4, PB_WG_DS4)
+PB_WGMMA(80, 40, 41, 42, PB_WG_RS5, PB_WG_DS5)
+PB_WGMMA(96, 48, 49, 50, PB_WG_RS6, PB_WG_DS6)
+PB_WGMMA(112, 56, 57, 58, PB_WG_RS7, PB_WG_DS7)
+PB_WGMMA(128, 64, 65, 66, PB_WG_RS8, PB_WG_DS8)
+PB_WGMMA(144, 72, 73, 74, PB_WG_RS9, PB_WG_DS9)
+PB_WGMMA(160, 80, 81, 82, PB_WG_RS10, PB_WG_DS10)
+PB_WGMMA(176, 88, 89, 90, PB_WG_RS11, PB_WG_DS11)
+PB_WGMMA(192, 96, 97, 98, PB_WG_RS12, PB_WG_DS12)
+PB_WGMMA(208, 104, 105, 106, PB_WG_RS13, PB_WG_DS13)
+PB_WGMMA(224, 112, 113, 114, PB_WG_RS14, PB_WG_DS14)
+PB_WGMMA(240, 120, 121, 122, PB_WG_RS15, PB_WG_DS15)
+PB_WGMMA(256, 128, 129, 130, PB_WG_RS16, PB_WG_DS16)
 }  // namespace pb

@@ -5,7 +5,7 @@
 //   * conv1 7x7 / stride 2 / pad 3 (3 -> 64) + BN + ReLU                   -> pb_resnet_stem7x7
 //   * MaxPool2d(3, stride 2, padding 1)                                    -> pb_maxpool3x3s2
 //   * AdaptiveAvgPool2d(1) + Linear(2048 -> n_out) + Sigmoid               -> pb_avgpool_fc_sigmoid
-// The bottleneck stacks run on the tcgen05 conv kernels (res_before_act = 1, 1x1 stride-2 downsample convs).
+// The bottleneck stacks run on the wgmma conv kernels (res_before_act = 1, 1x1 stride-2 downsample convs).
 // These four are 0.24 of the network's 4.1 GFLOP per frame; CUDA-core code, HBM / FMA bound.
 #include "internal.h"
 #include "ptx.cuh"

@@ -1,10 +1,10 @@
-"""torchvision ResNet50 court-keypoint regressor on the B200 kernels: the `model_type="resnet"` branch of
+"""torchvision ResNet50 court-keypoint regressor on the project's CUDA kernels: the `model_type="resnet"` branch of
 /root/reference/trackers/keypoints_tracker/keypoints_tracker.py:158-167 (model: resnet50 with fc -> 2 * 12 outputs),
 :276-312 (forward, sigmoid, scaling by the frame size) and keypoints_tracker/iterable.py:10-41 (BGR -> RGB, PIL
 Resize((224, 224)) = Image.BILINEAR, ToTensor, Normalize).
 
 Layers: pre-processing (Pillow-exact bilinear resize on device, normalise), conv1 7x7/s2 + maxpool (CUDA cores,
-csrc/resnet_aux.cu), the 16 bottlenecks as 52 fused conv launches on the tcgen05 kernels (BN folded, identity added
+csrc/resnet_aux.cu), the 16 bottlenecks as 52 fused conv launches on the wgmma conv kernels (BN folded, identity added
 before the ReLU in the epilogue, 1x1 stride-2 downsample convs), global average pool + fc + sigmoid.
 State-dict key names are torchvision's (`layer1.0.conv1.weight`, `fc.weight`, ...), so real checkpoints load.
 """

@@ -1,4 +1,4 @@
-"""TrackNet (ball heat-map U-Net) on the B200 conv kernels + the fused ball pipeline.
+"""TrackNet (ball heat-map U-Net) on the wgmma conv kernels + the fused ball pipeline.
 
 Replaces `self.tracknet` of the reference BallTracker (/root/reference/trackers/ball_tracker/ball_tracker.py:260-266,
 called at :445-446) and, through `BallPipeline`, the surrounding CPU stages:
@@ -62,7 +62,7 @@ class TrackNetEngine:
                                    sd[f"{p}.bn.running_var"].float(), 1e-5)
                 self._w[p] = ops.pack_conv_weight(w, b, ops.pad16(ci) if ci != 27 else 32, cout, self.device)
         # predictor 1x1 (64 -> 8) + sigmoid.  Default: a 1x1 tensor-core conv (fp16 weights, N = 16) writing the fp32
-        # NCHW planes -- HBM-bound at ~4.8 TB/s, 158 us per 32 frames.  PADEL_B200_TRACKNET_HEAD=pointwise selects the
+        # NCHW planes -- HBM-bound.  PADEL_B200_TRACKNET_HEAD=pointwise selects the
         # CUDA-core kernel with fp32 weights instead (308 us: ~800 instructions per 32 pixels, issue-bound).  The
         # fused-epilogue variant of the conv kernel also exists but costs more (512 FMAs per pixel in the epilogue).
         self._head_w = sd["predictor.weight"].float().reshape(8, 64).contiguous().to(self.device)

@@ -1,4 +1,4 @@
-"""YOLOv8 detect / pose inference on the B200 kernels behind the `ultralytics.YOLO(...).predict()` surface the
+"""YOLOv8 detect / pose inference on the project's CUDA kernels behind the `ultralytics.YOLO(...).predict()` surface the
 reference trackers use:
     /root/reference/trackers/players_tracker/players_tracker.py:303,338-339,351-359
     /root/reference/trackers/players_keypoints_tracker/players_keypoints_tracker.py:238,285-292

@@ -1,5 +1,5 @@
 """Drop-in tracker classes (same names / constructor arguments / results API as /root/reference/trackers/__init__.py:1-6)
-whose model forwards run on the B200 engine."""
+whose model forwards run on the CUDA engine."""
 from .players_tracker import Player, Players, PlayerTracker
 from .ball_tracker import Ball, BallTracker
 from .keypoints_tracker import Keypoint, Keypoints, KeypointsTracker

@@ -1,4 +1,4 @@
-"""BallTracker on the B200 engine — API of /root/reference/trackers/ball_tracker/ball_tracker.py (Ball :139-206,
+"""BallTracker on the CUDA engine — API of reference trackers/ball_tracker/ball_tracker.py (Ball :139-206,
 BallTracker :208-711).  The TrackNet stage (:373-523) runs fully on device through engine.BallPipeline.
 
 Documented deviations from reference quirks (SURVEY App. E):

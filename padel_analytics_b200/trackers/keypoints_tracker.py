@@ -1,4 +1,4 @@
-"""KeypointsTracker (court, 12 keypoints) on the B200 engine — API of
+"""KeypointsTracker (court, 12 keypoints) on the CUDA engine — API of
 /root/reference/trackers/keypoints_tracker/keypoints_tracker.py (:18-315): model_type="yolo" (YOLOv8-pose, predict_sample),
 model_type="resnet" (torchvision ResNet50 regressor :158-167, predict_frames :276-312, input pipeline
 keypoints_tracker/iterable.py:10-41) and the fixed-keypoints short-circuit."""

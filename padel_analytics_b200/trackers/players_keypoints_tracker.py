@@ -1,4 +1,4 @@
-"""PlayerKeypointsTracker on the B200 engine — API of
+"""PlayerKeypointsTracker on the CUDA engine — API of
 /root/reference/trackers/players_keypoints_tracker/players_keypoints_tracker.py (:15-327)."""
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""PlayerTracker on the B200 engine — same API as /root/reference/trackers/players_tracker/players_tracker.py
+"""PlayerTracker on the CUDA engine — same API as reference trackers/players_tracker/players_tracker.py
 (Player :14-197, Players :199-263, PlayerTracker :266-383)."""
 from __future__ import annotations
 

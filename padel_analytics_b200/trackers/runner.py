@@ -212,7 +212,7 @@ class TrackingRunner:
         import gc
 
         # The pass creates hundreds of small result objects per frame and keeps them all (the reference's results API);
-        # none of them form cycles, so the cyclic collector only costs time (measured: +30 % on a 4096-frame job as
+        # none of them form cycles, so the cyclic collector only costs time (more and more as
         # its generations fill up).  Collection is suspended for the duration of the pass.
         gc_was_on = gc.isenabled()
         gc.disable()

@@ -14,7 +14,7 @@ visibility is not itself borderline within 0.5 px), and every detection of ours 
 (no extras).  One more clause concerns the BOX of a SURE candidate: the seeded random checkpoints have multi-modal DFL
 distributions whose expectation (the box edge) is ill-conditioned; a box whose predicted IoU loss under 11-bit-mantissa
 logit noise exceeds 1 - 0.99 (dfl_edge_moves) is held to IoU >= 0.95 instead of 0.99 -- still the same box, but its
-edges are not determined to 1 % by the reference's own TF32 GPU arithmetic either (profiles/r02_parity_noise_floor.md).
+edges are not determined to 1 % by the reference's own TF32 GPU arithmetic either.
 The counts of each class are reported so that vacuity is visible.
 """
 from __future__ import annotations
@@ -49,8 +49,8 @@ def dfl_edge_moves(dfl_logits: torch.Tensor, strides: torch.Tensor, eps_logit: f
     of (move / box side) -- evaluated by compare_image on the box as reported (clipped to the image).  The seeded random checkpoints have i.i.d. DFL logits, i.e. multi-modal distributions with mass
     on far-apart bins (|i - E| ~ 5): such edges move by a pixel for a logit error of 1e-2, which no 11-bit-mantissa
     pipeline avoids -- the engine's fp16 storage, and equally the TF32 convolutions of the reference's own GPU path
-    (profiles/r02_parity_noise_floor.md).  A trained DFL head is unimodal (|i - E| < 1 where the mass is).
-    Calibration (scripts/emulate_engine_numerics.py, 440 boxes): actual loss / this predictor at eps = 1 has median
+    A trained DFL head is unimodal (|i - E| < 1 where the mass is).
+    Calibration (a CPU emulation of the engine's fp16 storage, 440 boxes): actual loss / this predictor at eps = 1 has median
     0.017, p99 0.056, max 0.09, uniformly over the three strides; the default eps_logit = 0.06 (3.5 x the median)
     flags 46 % of those boxes, among them all 24 that missed 0.99 in the emulation (at 0.04, 3 of them -- and one on
     the GPU, IoU 0.9888 -- slipped through).

@@ -1,4 +1,4 @@
-"""Engines (full networks on the tcgen05 conv kernel) vs the fp32 CPU oracle, and tracker-level parity.
+"""Engines (full networks on the wgmma conv kernels) vs the fp32 CPU oracle, and tracker-level parity.
 Tolerances: activations are stored in fp16 (10-bit mantissa, like the TF32 the reference's cuDNN path uses) with
 fp32 accumulation; the north-star acceptance bar is per-box IoU >= 0.99 and keypoint L2 < 0.5 px."""
 import numpy as np
@@ -197,7 +197,7 @@ def test_yolo_engine_predict_is_a_drop_in_for_ultralytics_predict(kind, src):
 
 def test_resnet50_court_regressor_matches_torchvision_oracle():
     """KeypointsTracker(model_type="resnet") (keypoints_tracker.py:158-167,276-312): the torchvision ResNet50 on the
-    B200 kernels vs torchvision itself on the CPU through the reference's input pipeline (iterable.py:10-41).
+    CUDA kernels vs torchvision itself on the CPU through the reference's input pipeline (iterable.py:10-41).
     Pre-processing is bit-exact (Pillow bilinear); the network output is compared in frame pixels."""
     from oracle import resnet as OR
     from padel_analytics_b200.engine.resnet_engine import ResNet50Engine
