@@ -304,20 +304,24 @@ constexpr int kConvAccRegs = 128;   // fp32 accumulators per consumer thread: S 
 constexpr int kEpiScratchPitch = 36;  // floats per scratch row (32 + 4 spreads the fragment stores over the banks)
 constexpr int kEpiScratchFloats = 16 * kEpiScratchPitch;  // per consumer warp
 
-template <int kU>
-__device__ __forceinline__ void epi_frag_store(const float (&acc)[kConvAccRegs], float* scr, int lane) {
-  const int r0 = lane >> 2, q = lane & 3;
+template <int kU, int kAcc>
+__device__ __forceinline__ void epi_frag_store(const float (&acc)[kAcc], float* scr, int lane) {
+  if constexpr (16 * kU < kAcc) {
+    const int r0 = lane >> 2, q = lane & 3;
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    *reinterpret_cast<float2*>(scr + r0 * kEpiScratchPitch + 8 * i + 2 * q) =
-        make_float2(acc[16 * kU + 4 * i], acc[16 * kU + 4 * i + 1]);
-    *reinterpret_cast<float2*>(scr + (r0 + 8) * kEpiScratchPitch + 8 * i + 2 * q) =
-        make_float2(acc[16 * kU + 4 * i + 2], acc[16 * kU + 4 * i + 3]);
+    for (int i = 0; i < 4; ++i) {
+      *reinterpret_cast<float2*>(scr + r0 * kEpiScratchPitch + 8 * i + 2 * q) =
+          make_float2(acc[16 * kU + 4 * i], acc[16 * kU + 4 * i + 1]);
+      *reinterpret_cast<float2*>(scr + (r0 + 8) * kEpiScratchPitch + 8 * i + 2 * q) =
+          make_float2(acc[16 * kU + 4 * i + 2], acc[16 * kU + 4 * i + 3]);
+    }
   }
 }
 
-// chunk u of the accumulators -> this lane's 16 channels
-__device__ __forceinline__ void epi_transpose16(const float (&acc)[kConvAccRegs], int u, float* scr, int lane,
+// chunk u of the accumulators -> this lane's 16 channels.  With a compile-time u (unrolled caller) the switch folds
+// to one case.
+template <int kAcc>
+__device__ __forceinline__ void epi_transpose16(const float (&acc)[kAcc], int u, float* scr, int lane,
                                                 uint32_t (&r)[16]) {
   __syncwarp();  // the previous chunk's reads are done
   switch (u) {  // CTA-uniform; the accumulator index has to be a compile-time constant
@@ -408,20 +412,28 @@ __device__ __forceinline__ void epi_unit(const ConvKParams& kp, const EpiPix& px
 
 // One consumer warp's tile; pix_of(j, pool_writer) = this lane's pixel in sub-tile j.  Every lane runs every chunk
 // (the butterfly shuffles); the fused head adds the half-pixel sums of lanes l and l ^ 16.
-template <int kEpi, typename PixOf>
-__device__ __forceinline__ void epilogue_tile(const ConvKParams& kp, const float (&acc)[kConvAccRegs], int S, int nt,
+// kS / kNch > 0: sub-tiles / 32-column chunks per sub-tile known at compile time (the halo kernel) -- both loops unroll
+// and every accumulator index is a constant; 0: taken from S / kp.BN at run time (the per-tap kernel).
+template <int kEpi, int kS = 0, int kNch = 0, int kAcc, typename PixOf>
+__device__ __forceinline__ void epilogue_tile(const ConvKParams& kp, const float (&acc)[kAcc], int S, int nt,
                                               const float* __restrict__ sbias, float* scr, int lane, PixOf pix_of) {
-  const int nch = (kp.BN + 31) >> 5;
+  const int nch = kNch > 0 ? kNch : (kp.BN + 31) >> 5;
   const bool fast = kEpi != PB_EPI_GENERIC || epilogue_fast_ok(kp);  // the host picks a plain class only when it holds
   const int col0 = 16 * (lane >> 4);
-  for (int j = 0; j < S; ++j) {
+  auto sub_tile = [&](int j) {
     bool pool_writer = false;
     const EpiPix px = pix_of(j, pool_writer);
     float hacc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};  // fused 1x1 head partial sums
-    for (int c = 0; c < nch; ++c) {
+    auto chunk = [&](int c) {
       uint32_t r[16];
       epi_transpose16(acc, j * nch + c, scr, lane, r);
       epi_unit<kEpi>(kp, px, pool_writer, nt, 32 * c + col0, r, sbias, fast, hacc);
+    };
+    if constexpr (kNch > 0) {
+#pragma unroll
+      for (int c = 0; c < kNch; ++c) chunk(c);
+    } else {
+      for (int c = 0; c < nch; ++c) chunk(c);
     }
     if (kEpi == PB_EPI_GENERIC && !fast && kp.head_n > 0) {
 #pragma unroll
@@ -434,16 +446,22 @@ __device__ __forceinline__ void epilogue_tile(const ConvKParams& kp, const float
           if (q < kp.head_n) ho[(size_t)q * plane] = __fdividef(1.f, 1.f + __expf(-(hacc[q] + __ldg(kp.head_b + q))));
       }
     }
+  };
+  if constexpr (kS > 0) {
+#pragma unroll
+    for (int j = 0; j < kS; ++j) sub_tile(j);
+  } else {
+    for (int j = 0; j < S; ++j) sub_tile(j);
   }
 }
 
 // acc (+)= A * B^T over kSteps k-steps of 16 for the warpgroup's 64 rows of kS sub-tiles (A descriptors sub_units
 // apart); accum = 0 overwrites.  kN = the N tile, a compile-time constant of the instruction.
-template <int kN, int kS, int kSteps>
-__device__ __forceinline__ void mma_n(float (&acc)[kConvAccRegs], uint64_t ad, uint64_t sub_units, uint64_t bd,
+template <int kN, int kS, int kSteps, int kAcc>
+__device__ __forceinline__ void mma_n(float (&acc)[kAcc], uint64_t ad, uint64_t sub_units, uint64_t bd,
                                       uint32_t accum) {
   constexpr int kAS = (kN + 31) / 32 * 16;
-  if constexpr (kS * kAS <= kConvAccRegs) {
+  if constexpr (kS * kAS <= kAcc) {
 #pragma unroll
     for (int j = 0; j < kS; ++j)
 #pragma unroll

@@ -1,0 +1,236 @@
+// The halo conv kernel (conv_halo_kernel) and the lookup of its instantiations; the host set-ups live in
+// conv_halo.cu.  Each epilogue class is instantiated in a translation unit of its own (conv_halo_inst_*.cu) so that the
+// several hundred (S, k-steps, N) variants compile in parallel.
+#pragma once
+#include "conv_common.cuh"
+#include "internal.h"
+#include "ptx.cuh"
+
+namespace pb {
+
+constexpr int kHaloMaxA = 4;
+constexpr int kHaloMaxB = 12;
+
+struct HaloSmemTail {
+  uint64_t a_full[kHaloMaxA];
+  uint64_t a_empty[kHaloMaxA];
+  uint64_t b_full[kHaloMaxB];
+  uint64_t b_empty[kHaloMaxB];
+  float bias[kConvMaxCout];
+  float scratch[kConvConsumerWarps * kEpiScratchFloats];  // epilogue transposition, one slice per consumer warp
+};
+
+struct HaloTile {
+  int tw, th, n;
+};
+__device__ __forceinline__ HaloTile halo_decode(const ConvKParams& kp, int tile) {
+  HaloTile t;
+  int q;
+  fast_divmod(q, t.tw, tile, kp.fd_w);
+  fast_divmod(t.n, t.th, q, kp.fd_h);
+  return t;
+}
+
+// kS (sub-tiles), kSteps (16-element k-steps per channel block) and kBN (the N tile = cout_pad) are compile-time so
+// the wgmma issue loop is straight-line code with immediate descriptor offsets, the accumulator array holds exactly
+// the kS * ceil(kBN / 32) * 16 registers this layer needs, and the epilogue indexes it with constants.  One
+// instantiation per N keeps ptxas from reserving registers for the widest case, which would serialise the wgmmas
+// (no group in flight while the next is issued) and spill.
+template <int kS, int kSteps, int kBN, int kEpi>
+__global__ void __launch_bounds__(kConvThreads, 1)
+conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
+                 const __grid_constant__ ConvKParams kp) {
+  constexpr int kNch = (kBN + 31) / 32;  // 32-column epilogue chunks per sub-tile
+  constexpr int kAcc = kS * kNch * 16;   // fp32 accumulators per consumer thread
+  static_assert(kAcc <= kConvAccRegs, "accumulators of kS sub-tiles must fit the registers");
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* a_base = smem;
+  uint8_t* b_base = smem + (size_t)kp.a_stages * kp.a_bytes;
+  HaloSmemTail* tail = reinterpret_cast<HaloSmemTail*>(b_base + (size_t)kp.b_stages * kp.b_bytes);
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  constexpr int S = kS;
+  const int G = kp.hs_G;
+  const uint32_t row_bytes = (uint32_t)kp.KB * 2u;       // weight rows (and activation rows unless stride 2)
+  const uint32_t a_row_bytes = kp.hs_a_row_bytes;        // activation (halo) rows
+  const int tap_groups = kp.hs_ntaps / G;
+
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&tmap_a);
+    for (int i = 0; i < kp.a_stages; ++i) {
+      mbar_init(&tail->a_full[i], 1);
+      mbar_init(&tail->a_empty[i], kConvConsumerWarps);
+    }
+    for (int i = 0; i < kp.b_stages; ++i) {
+      mbar_init(&tail->b_full[i], 1);
+      mbar_init(&tail->b_empty[i], kConvConsumerWarps);
+    }
+    fence_mbar_init();
+  }
+  if (warp == 1 && lane == 0) tma_prefetch_desc(&tmap_w);
+  for (int i = threadIdx.x; i < kp.cout_pad; i += blockDim.x) tail->bias[i] = kp.bias[i];
+  __syncthreads();
+  // PDL: the prologue above touched constant data only; from here on activations are read and written.  The weight
+  // producer (warp 1) reads constants only and starts fetching while the previous kernel is still running.
+  griddep_launch_dependents();
+  if (warp != 1) griddep_wait();
+
+  if (warp < 4) {
+    warpgroup_reg_dealloc<kConvProducerRegs>();
+    if (warp == 0 && lane == 0) {
+      // ===================== halo producer: one TMA box per (tile, channel block) =====================
+      int st = 0;
+      uint32_t ph = 0;
+      for (int tile = blockIdx.x; tile < kp.total_tiles; tile += gridDim.x) {
+        const HaloTile t = halo_decode(kp, tile);
+        for (int cb = 0; cb < kp.kblocks; ++cb) {
+          mbar_wait(&tail->a_empty[st], ph ^ 1);
+          mbar_arrive_expect_tx(&tail->a_full[st], kp.halo_bytes);
+          tma_load_5d(a_base + (size_t)st * kp.a_bytes, &tmap_a, &tail->a_full[st], kp.c_in_off + cb * kp.KB,
+                      t.tw * 8 * S + kp.hs_x0, 0, t.th * 16 + kp.hs_y0, t.n);
+          if (++st == kp.a_stages) {
+            st = 0;
+            ph ^= 1;
+          }
+        }
+      }
+    } else if (warp == 1 && lane == 0) {
+      // ===================== weight producer: one TMA box per (channel block, tap group) =====================
+      // Resident mode (kp.b_resident: the whole filter bank fits next to the halo ring): every box is fetched ONCE per
+      // CTA and reused by all its tiles -- without it a small-channel layer re-reads its weights from L2 for every
+      // tile, as many bytes as the activations themselves.
+      int st = 0;
+      uint32_t ph = 0;
+      for (int tile = blockIdx.x; tile < kp.total_tiles; tile += gridDim.x) {
+        for (int cb = 0; cb < kp.kblocks; ++cb) {
+          for (int tg = 0; tg < tap_groups; ++tg) {
+            if (!kp.b_resident) mbar_wait(&tail->b_empty[st], ph ^ 1);
+            mbar_arrive_expect_tx(&tail->b_full[st], kp.b_tx_bytes);
+            tma_load_3d(b_base + (size_t)st * kp.b_bytes, &tmap_w, &tail->b_full[st], cb * kp.KB, 0, tg * G);
+            if (++st == kp.b_stages) {
+              st = 0;
+              ph ^= 1;
+            }
+          }
+        }
+        if (kp.b_resident) break;
+      }
+    }
+    return;
+  }
+
+  // ===================== consumers: wgmma + epilogue =====================
+  // A sub-tile is 16 image rows x 8 columns = 128 pixels (row m = 8 * image row + column); warpgroup g computes its
+  // image rows 8g .. 8g + 7, i.e. the 8-row groups 8g .. 8g + 7 of every tap's A descriptor.
+  warpgroup_reg_alloc<kConvConsumerRegs>();
+  const int cw = warp - 4, g = cw >> 2, wq = cw & 3;
+  float* scr = tail->scratch + cw * kEpiScratchFloats;
+  const uint32_t sbo = (uint32_t)kp.hs_sbo_rows * a_row_bytes;
+  const uint64_t g_units = (uint64_t)((8u * (uint32_t)g * sbo) >> 4);
+  const uint32_t tap_b_units = ((uint32_t)kBN * row_bytes) >> 4;               // 16-byte units
+  const uint64_t sub_units = (uint64_t)((8u * a_row_bytes) >> 4);              // next sub-tile: +8 pixels
+  const int m = 64 * g + 16 * wq + (lane & 15);  // this lane's pixel of each sub-tile in the epilogue
+  const int row = m >> 3, col = m & 7;
+  float acc[kAcc];
+#pragma unroll
+  for (int i = 0; i < kAcc; ++i) acc[i] = 0.f;
+  int ast = 0, bst = 0;
+  uint32_t aph = 0, bph = 0;
+  for (int tile = blockIdx.x; tile < kp.total_tiles; tile += gridDim.x) {
+    const HaloTile t = halo_decode(kp, tile);
+    // One group of wgmmas (one weight stage) stays in flight while the next is issued: a weight stage is released
+    // once the group after it has been issued and wgmma_wait<1> has retired it, a halo stage once the first group
+    // of the next channel block has (prev_b / prev_a: the stages still read by the group in flight, -1 = none).
+    int prev_b = -1, prev_a = -1;
+    for (int cb = 0; cb < kp.kblocks; ++cb) {
+      mbar_wait(&tail->a_full[ast], aph);
+      // Descriptor arithmetic is hoisted: per (channel block, weight stage) one base descriptor each; taps,
+      // sub-tiles and k-steps only add precomputed 16-byte-unit offsets to the low word.
+      const uint64_t a_desc0 = wgmma_desc(smem_u32(a_base + (size_t)ast * kp.a_bytes), a_row_bytes, sbo) + g_units;
+      for (int tg = 0; tg < tap_groups; ++tg) {
+        mbar_wait(&tail->b_full[bst], kp.b_resident ? 0u : bph);  // resident: filled once, phase 0 stays complete
+        const uint64_t b_desc0 = wgmma_desc_kmajor(smem_u32(b_base + (size_t)bst * kp.b_bytes), row_bytes);
+        wgmma_fence();
+        for (int ti = 0; ti < G; ++ti) {
+          const int tap = tg * G + ti;
+          mma_n<kBN, kS, kSteps>(acc, a_desc0 + (uint64_t)(uint32_t)kp.hs_tap_desc[tap], sub_units,
+                                 b_desc0 + (uint64_t)((uint32_t)ti * tap_b_units), (uint32_t)((cb | tap) != 0));
+        }
+        wgmma_commit();
+        if (prev_b >= 0) {
+          wgmma_wait<1>();
+          if (!kp.b_resident) consumer_release(&tail->b_empty[prev_b], lane);
+          if (prev_a >= 0) consumer_release(&tail->a_empty[prev_a], lane);
+          prev_a = -1;
+        }
+        prev_b = bst;
+        if (++bst == kp.b_stages) {
+          bst = 0;
+          bph ^= 1;
+        }
+      }
+      prev_a = ast;
+      if (++ast == kp.a_stages) {
+        ast = 0;
+        aph ^= 1;
+      }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_operands(acc);
+    if (!kp.b_resident) consumer_release(&tail->b_empty[prev_b], lane);
+    consumer_release(&tail->a_empty[prev_a], lane);
+    const int oh = t.th * 16 + row, ow0 = t.tw * 8 * S + col;
+    epilogue_tile<kEpi, kS, kNch>(kp, acc, S, 0, tail->bias, scr, lane, [&](int j, bool& pool_writer) {
+      EpiPix px;
+      px.n = t.n;
+      px.oh = oh;
+      px.ow = ow0 + 8 * j;
+      px.valid = (px.ow < kp.Wo) && (px.oh < kp.Ho);
+      px.pix = ((size_t)px.n * kp.Ho + px.oh) * kp.Wo + px.ow;
+      pool_writer = ((row | col) & 1) == 0;
+      return px;
+    });
+  }
+}
+
+typedef void (*HaloKernelFn)(CUtensorMap, CUtensorMap, ConvKParams);
+
+// Instantiations: every N tile a halo set-up can produce (cout_pad = 16 .. 256 in steps of 16) with every sub-tile
+// count whose accumulators fit (S * ceil(N / 32) * 16 <= kConvAccRegs), for k-steps 1 / 2 / 4 (KB = 16 / 32 / 64).
+template <int kS, int kSteps, int kEpi>
+static HaloKernelFn halo_kernel_for_bn(int BN) {
+  switch (BN) {
+#define PB_HALO_BN(n_)                                                                     \
+  case n_:                                                                                 \
+    if constexpr (kS * ((n_ + 31) / 32) * 16 <= kConvAccRegs) return conv_halo_kernel<kS, kSteps, n_, kEpi>; \
+    break;
+    PB_HALO_BN(16) PB_HALO_BN(32) PB_HALO_BN(48) PB_HALO_BN(64) PB_HALO_BN(80) PB_HALO_BN(96) PB_HALO_BN(112)
+    PB_HALO_BN(128) PB_HALO_BN(144) PB_HALO_BN(160) PB_HALO_BN(176) PB_HALO_BN(192) PB_HALO_BN(208)
+    PB_HALO_BN(224) PB_HALO_BN(240) PB_HALO_BN(256)
+#undef PB_HALO_BN
+    default: break;
+  }
+  return nullptr;
+}
+
+template <int kEpi>
+HaloKernelFn halo_kernel_lookup(int S, int steps, int BN) {
+#define PB_HALO_CASE(s_, k_) \
+  if (S == s_ && steps == k_) return halo_kernel_for_bn<s_, k_, kEpi>(BN);
+  PB_HALO_CASE(1, 1) PB_HALO_CASE(1, 2) PB_HALO_CASE(1, 4)
+  PB_HALO_CASE(2, 1) PB_HALO_CASE(2, 2) PB_HALO_CASE(2, 4)
+  PB_HALO_CASE(4, 1) PB_HALO_CASE(4, 2) PB_HALO_CASE(4, 4)
+#undef PB_HALO_CASE
+  return nullptr;
+}
+
+
+// instantiated in conv_halo_inst_*.cu
+extern template HaloKernelFn halo_kernel_lookup<PB_EPI_GENERIC>(int, int, int);
+extern template HaloKernelFn halo_kernel_lookup<PB_EPI_SILU>(int, int, int);
+extern template HaloKernelFn halo_kernel_lookup<PB_EPI_RELU>(int, int, int);
+extern template HaloKernelFn halo_kernel_lookup<PB_EPI_SILU_RES>(int, int, int);
+
+}  // namespace pb
