@@ -174,6 +174,22 @@ __device__ __forceinline__ void silu4(float& a, float& b, float& c, float& d) {
   d *= dc * rcd;
 }
 
+// silu4 on the wgmma fragment layout, where channels 4k .. 4k+3 of a pixel are split over lane l (two of them) and
+// lane l ^ 1 (the other two).  Each lane forms its pair's product of denominators, swaps it with lane l ^ 1 and
+// finishes its two values with the operations silu4 applies to them, so the results are bit-identical (the product
+// of the two pair products is commutative).  Every lane of the warp must call it.
+__device__ __forceinline__ void silu2_frag(float& a, float& b) {
+  constexpr float kNegLog2e = -1.4426950408889634f;
+  const float da = 1.f + ex2_approx(fminf(a * kNegLog2e, 30.f));
+  const float db = 1.f + ex2_approx(fminf(b * kNegLog2e, 30.f));
+  const float p = da * db;
+  const float po = __shfl_xor_sync(0xffffffffu, p, 1);
+  const float r = rcp_approx(p * po);
+  const float rp = po * r;  // 1 / (da db)
+  a *= db * rp;
+  b *= da * rp;
+}
+
 // Where one thread's 16-channel chunk goes: byte pointer of the pixel (channel 0 of the N tile), byte strides of the
 // 2x2 replication (UP2 only) and the number of channels of this chunk that exist (fp32 heads may end mid-chunk).
 struct EpiOut {

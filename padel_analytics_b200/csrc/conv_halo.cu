@@ -25,10 +25,82 @@ namespace pb {
 // returns -1 (no error) when the layer should use the per-tap kernel.
 // ------------------------------------------------------------------------------------------------------------
 
+// shared memory for the rings and the staging tile (the tail and the alignment slack come on top, <= 227 KB)
+constexpr size_t kHaloSmemBudget = 196 * 1024;
+
+// TMA-store epilogue (conv_halo_kernel.cuh::halo_epilogue_tma) for an fp16 output without residual whose N tile is
+// stored whole: the staging tile (S * BN * 256 bytes) joins the rings inside the budget -- the weight ring down to four,
+// then the halo ring down to two, then the weight ring down to three stages; S and G stay as chosen.  Layers where it
+// does not fit, or does not apply, keep the per-lane store epilogue.  PADEL_B200_CONV_TMA_STORE=0 disables it (A/B).
+static int halo_plan_store(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode) {
+  const size_t budget = kHaloSmemBudget;
+  static const int enabled = [] {
+    const char* e = getenv("PADEL_B200_CONV_TMA_STORE");
+    return e ? atoi(e) : 1;
+  }();
+  ConvKParams& kp = plan->kp;
+  kp.st_bytes = 0;
+  kp.st_maps = 0;
+  kp.st_pool = 0;
+  const bool f16 = d->out_mode == PB_OUT_F16_NHWC || d->out_mode == PB_OUT_F16_NHWC_UP2;
+  if (!enabled || kp.dbg_flags != 0 || d->res || d->head_n != 0 || !f16 || plan->epi == PB_EPI_SILU_RES ||
+      d->cout_store != kp.BN || ((d->out_C | d->out_coff) & 7) != 0)
+    return 0;
+  // Deep-K streamed layers (more than two channel blocks) are mainloop-bound and need their third halo stage and
+  // deep weight ring more than an asynchronous epilogue (H100: up_block_2.conv_1 of TrackNet ran 5 % slower with it).
+  if (!kp.b_resident && kp.kblocks > 2) return 0;
+  const uint32_t st = (uint32_t)kp.hs_S * (uint32_t)kp.BN * 256u;
+  int as = kp.a_stages, bs = kp.b_stages;
+  auto total = [&] { return (size_t)as * kp.a_bytes + (size_t)bs * kp.b_bytes + st; };
+  while (total() > budget) {
+    if (!kp.b_resident && bs > 4) --bs;
+    else if (as > 2) --as;
+    else if (!kp.b_resident && bs > 3) --bs;
+    else return 0;
+  }
+  // one map per destination of the staging box (channels, 8S columns, 8 rows, image); base = channel 0 of the slice
+  const int S = kp.hs_S, bc = halo_store_box_channels(kp.BN);
+  const CUtensorMapSwizzle swz = bc == 64 ? CU_TENSOR_MAP_SWIZZLE_128B
+                                 : bc == 32 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                            : CU_TENSOR_MAP_SWIZZLE_32B;
+  int nm = 0;
+  auto add = [&](void* out, int C, int coff, int W, int H, int up, int dy, int dx, int bw, int bh) {
+    const size_t pxb = (size_t)C * 2;
+    char* base = reinterpret_cast<char*>(out) + ((size_t)(dy * up * W + dx) * C + coff) * 2;
+    cuuint64_t dims[4] = {(cuuint64_t)kp.BN, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)kp.N};
+    cuuint64_t strides[3] = {up * pxb, (cuuint64_t)up * up * W * pxb, (cuuint64_t)up * up * W * H * pxb};
+    cuuint32_t box[4] = {(cuuint32_t)bc, (cuuint32_t)bw, (cuuint32_t)bh, 1};
+    cuuint32_t estr[4] = {1, 1, 1, 1};
+    return encode(&plan->tmap_o.m[nm++], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, base, dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  };
+  CUresult r = CUDA_SUCCESS;
+  const int up = d->out_mode == PB_OUT_F16_NHWC_UP2 ? 2 : 1;
+  for (int dy = 0; dy < up; ++dy)
+    for (int dx = 0; dx < up; ++dx)
+      if (r == CUDA_SUCCESS) r = add(d->out, d->out_C, d->out_coff, kp.Wo, kp.Ho, up, dy, dx, 8 * S, 8);
+  if (d->out2_mode == PB_OUT2_UP2) {
+    for (int dy = 0; dy < 2; ++dy)
+      for (int dx = 0; dx < 2; ++dx)
+        if (r == CUDA_SUCCESS) r = add(d->out2, d->out2_C, d->out2_coff, kp.Wo, kp.Ho, 2, dy, dx, 8 * S, 8);
+  }
+  kp.st_maps = nm;
+  if (d->out2_mode == PB_OUT2_POOL2 && r == CUDA_SUCCESS) {
+    r = add(d->out2, d->out2_C, d->out2_coff, kp.Wo / 2, kp.Ho / 2, 1, 0, 0, 4 * S, 4);
+    kp.st_pool = 1;
+  }
+  PB_CHECK(r == CUDA_SUCCESS, "conv(halo): cuTensorMapEncodeTiled(store) failed with %d", (int)r);
+  kp.st_bytes = st;
+  kp.a_stages = as;
+  kp.b_stages = bs;
+  return 0;
+}
+
 // Launch configuration shared by the halo set-ups: one persistent CTA per SM.
 static void halo_finish_config(ConvPlan* plan) {
   const ConvKParams& kp = plan->kp;
-  plan->smem_bytes = (size_t)kp.a_stages * kp.a_bytes + (size_t)kp.b_stages * kp.b_bytes + sizeof(HaloSmemTail) + 1024;
+  plan->smem_bytes = (size_t)kp.a_stages * kp.a_bytes + (size_t)kp.b_stages * kp.b_bytes + kp.st_bytes +
+                     sizeof(HaloSmemTail) + 1024;
   plan->threads = kConvThreads;
   plan->grid = kp.total_tiles < num_sms() ? kp.total_tiles : num_sms();
 }
@@ -90,6 +162,7 @@ int conv_stem_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode)
   kp.tiles_h = (kp.Ho + 15) / 16;
   kp.tiles_n = kp.N;
   kp.total_tiles = kp.tiles_w * kp.tiles_h * kp.tiles_n;
+  if (halo_plan_store(d, plan, encode) != 0) return 1;
   halo_finish_config(plan);
   plan->variant = 1;
   {
@@ -134,7 +207,7 @@ int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode)
   const int BN = d->cout_pad;
   const uint32_t row_bytes = (uint32_t)kp.KB * 2u;
   const int acc_cols = (BN + 31) / 32 * 32;
-  const size_t budget = 196 * 1024;
+  const size_t budget = kHaloSmemBudget;
   // Choose S (sub-tiles per CTA tile: fewer halo + weight bytes per pixel) first, then G (taps per weight box:
   // fewer TMA operations) as large as shared memory allows.
   const uint32_t tap_bytes = (uint32_t)BN * row_bytes;
@@ -225,6 +298,7 @@ int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode)
   kp.tiles_h = (kp.Ho + 15) / 16;
   kp.tiles_n = kp.N;
   kp.total_tiles = kp.tiles_w * kp.tiles_h * kp.tiles_n;
+  if (halo_plan_store(d, plan, encode) != 0) return 1;
   halo_finish_config(plan);
   plan->variant = 1;
 
@@ -275,7 +349,7 @@ int conv_halo_1x1_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn enc
   const int BN = d->cout_pad;
   const uint32_t row_bytes = (uint32_t)kp.KB * 2u;
   const int acc_cols = (BN + 31) / 32 * 32;
-  const size_t budget = 196 * 1024;
+  const size_t budget = kHaloSmemBudget;
   const uint32_t tap_bytes = (uint32_t)BN * row_bytes;
   const uint32_t res_box = (tap_bytes + 1023u) & ~1023u;
   const size_t res_total = (size_t)kp.kblocks * res_box;
@@ -319,6 +393,7 @@ int conv_halo_1x1_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn enc
   kp.tiles_h = (kp.Ho + 15) / 16;
   kp.tiles_n = kp.N;
   kp.total_tiles = kp.tiles_w * kp.tiles_h * kp.tiles_n;
+  if (halo_plan_store(d, plan, encode) != 0) return 1;
   halo_finish_config(plan);
   plan->variant = 1;
   const CUtensorMapSwizzle swz = kp.KB == 64   ? CU_TENSOR_MAP_SWIZZLE_128B
@@ -369,7 +444,7 @@ int conv_halo_s2_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn enco
   const int acc_cols = (BN + 31) / 32 * 32;
   const uint32_t tap_bytes = (uint32_t)BN * row_bytes;
   const uint32_t b_alloc = (9u * tap_bytes + 1023u) & ~1023u;  // all nine taps in one weight box
-  const size_t budget = 196 * 1024;
+  const size_t budget = kHaloSmemBudget;
   int S = 0;
   for (int s = 4; s >= 1; s >>= 1) {
     if (s * acc_cols > 2 * kConvAccRegs) continue;
@@ -411,6 +486,7 @@ int conv_halo_s2_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn enco
   kp.tiles_h = (kp.Ho + 15) / 16;
   kp.tiles_n = kp.N;
   kp.total_tiles = kp.tiles_w * kp.tiles_h * kp.tiles_n;
+  if (halo_plan_store(d, plan, encode) != 0) return 1;
   halo_finish_config(plan);
   plan->variant = 1;
   {
@@ -450,14 +526,19 @@ static HaloKernelFn halo_kernel_pick(const ConvPlan* plan) {
 
 int conv_halo_launch(const ConvPlan* plan, cudaStream_t stream) {
   const ConvKParams& kp = plan->kp;
+  const int tma_store = kp.st_bytes != 0;
   HaloKernelFn fn = halo_kernel_pick(plan);
-  PB_CHECK(fn != nullptr, "conv(halo): no kernel instantiation for S=%d, k-steps=%d, N=%d, epilogue class %d",
-           kp.hs_S, kp.KB / 16, kp.BN, plan->epi);
+  PB_CHECK(fn != nullptr,
+           "conv(halo): no kernel instantiation for S=%d, k-steps=%d, N=%d, epilogue class %d (TMA store %d)", kp.hs_S,
+           kp.KB / 16, kp.BN, plan->epi, tma_store);
   PB_CUDA((cudaError_t)ensure_dynamic_smem(reinterpret_cast<const void*>(fn), 227 * 1024));
   cudaError_t le = launch_ex(fn, dim3(plan->grid), dim3(plan->threads), plan->smem_bytes, stream, 1, plan->pdl != 0,
-                             plan->tmap_a, plan->tmap_w, plan->kp);
-  PB_CHECK(le == cudaSuccess, "conv(halo): launch failed: %s (grid %d, threads %d, smem %zu, tiles %d, S %d, BN %d, KB %d)",
-           cudaGetErrorString(le), plan->grid, plan->threads, plan->smem_bytes, kp.total_tiles, kp.hs_S, kp.BN, kp.KB);
+                             plan->tmap_a, plan->tmap_w, plan->kp, plan->tmap_o);
+  PB_CHECK(le == cudaSuccess,
+           "conv(halo): launch failed: %s (grid %d, threads %d, smem %zu, tiles %d, S %d, k-steps %d, N %d, epilogue "
+           "class %d, TMA store %d)",
+           cudaGetErrorString(le), plan->grid, plan->threads, plan->smem_bytes, kp.total_tiles, kp.hs_S, kp.KB / 16,
+           kp.BN, plan->epi, tma_store);
   count_launch();
   return 0;
 }

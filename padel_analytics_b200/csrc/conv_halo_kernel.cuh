@@ -31,6 +31,136 @@ __device__ __forceinline__ HaloTile halo_decode(const ConvKParams& kp, int tile)
   return t;
 }
 
+// Channels per TMA store box of the staging tile: its rows are one swizzle span (128 / 64 / 32 bytes).
+__host__ __device__ constexpr int halo_store_box_channels(int bn) { return bn % 64 == 0 ? 64 : (bn % 32 == 0 ? 32 : 16); }
+
+// TMA-store epilogue (kp.st_bytes != 0) of one consumer warpgroup: its 8 image rows x 8S columns x kBN channels.
+// Bias, activation and fp16 packing run on the accumulators in the wgmma fragment layout (channel 8i + 2(lane % 4),
+// pixel row lane / 4 and + 8 = image rows 2wq, 2wq + 1) with the fp32 operations of epi_compute16, so the values are
+// bit-identical to the per-lane store epilogue.  stmatrix writes them into the staging tile, laid out as TMA boxes
+// (channels, 8S columns, 8 rows) whose 16-byte chunks carry the store map's swizzle (no bank conflicts at any pixel
+// stride); one thread then issues the stores, and the warpgroup goes back to the next tile's wgmmas while the copy
+// engine writes.  PB_OUT2_POOL2: the 2x2 maxima are read back from the staged tile and reuse the staging area once
+// the primary stores have read it (no registers held across the accumulators).  TMA drops the parts of a box outside the tensor (edge tiles).
+template <int kEpi, int kS, int kBN, int kAcc>
+__device__ __forceinline__ void halo_epilogue_tma(const ConvKParams& kp, const HaloStoreMaps& maps,
+                                                  const float (&acc)[kAcc], const float* __restrict__ sbias,
+                                                  uint8_t* stage, const HaloTile& t, int g, int wq, int lane) {
+  constexpr int kAS = (kBN + 31) / 32 * 16;  // accumulators per sub-tile
+  constexpr int kBC = halo_store_box_channels(kBN);
+  constexpr uint32_t kRow = 2u * kBC;               // staging row = one pixel's kBC channels = the swizzle span
+  constexpr uint32_t kBox = 64u * kS * kRow;        // 8 rows x 8S columns
+  constexpr uint32_t kPoolBox = 16u * kS * kRow;    // 4 x 4S pooled pixels
+  constexpr int kCpr = kBC / 8;                     // 16-byte chunks per row
+  const int act = kEpi == PB_EPI_SILU ? PB_ACT_SILU : (kEpi == PB_EPI_RELU ? PB_ACT_RELU : kp.act);
+  const bool pool = kp.st_pool != 0;
+  const bool leader = (threadIdx.x & 127) == 0;
+  const int bar = 1 + g;  // named barrier of this warpgroup
+  const int q = lane & 3, mi = lane >> 3;
+  const uint32_t sbase = smem_u32(stage);
+  // stmatrix: lane l addresses row l % 8 (= pixel column) of matrix mi = l / 8 (image row + (mi & 1), channel chunk
+  // + (mi >> 1)).  Pixel index = image row * 8S + column, so the swizzle key (the pixel's 128-byte line mod the span)
+  // is a per-lane constant.
+  const uint32_t key = (((uint32_t)(lane & 7) * kRow) >> 7) & (uint32_t)(kCpr - 1);
+  const uint32_t lane_row = sbase + (uint32_t)((2 * wq + (mi & 1)) * 8 * kS + (lane & 7)) * kRow;
+  const uint32_t hi = (uint32_t)(mi >> 1);
+
+  if (leader) bulk_wait_group_read0();  // the previous tile's stores have read the staging area
+  named_barrier_sync(bar, 128);
+#pragma unroll
+  for (int j = 0; j < kS; ++j) {
+#pragma unroll
+    for (int i = 0; i < kBN / 8; i += 2) {  // 16 channels: fragment column blocks i, i + 1
+      uint32_t h[4];
+#pragma unroll
+      for (int u = 0; u < 2; ++u) {
+        const float* a4 = acc + j * kAS + 4 * (i + u);
+        const float2 b = *reinterpret_cast<const float2*>(sbias + 8 * (i + u) + 2 * q);
+        float v0 = a4[0] + b.x, v1 = a4[1] + b.y, v2 = a4[2] + b.x, v3 = a4[3] + b.y;
+        if (act == PB_ACT_SILU) {
+          silu2_frag(v0, v1);
+          silu2_frag(v2, v3);
+        } else if (act == PB_ACT_RELU) {
+          v0 = fmaxf(v0, 0.f);
+          v1 = fmaxf(v1, 0.f);
+          v2 = fmaxf(v2, 0.f);
+          v3 = fmaxf(v3, 0.f);
+        } else if (act == PB_ACT_SIGMOID) {
+          v0 = __fdividef(1.f, 1.f + __expf(-v0));
+          v1 = __fdividef(1.f, 1.f + __expf(-v1));
+          v2 = __fdividef(1.f, 1.f + __expf(-v2));
+          v3 = __fdividef(1.f, 1.f + __expf(-v3));
+        }
+        const __half2 top = __floats2half2_rn(v0, v1), bot = __floats2half2_rn(v2, v3);
+        h[2 * u] = *reinterpret_cast<const uint32_t*>(&top);
+        h[2 * u + 1] = *reinterpret_cast<const uint32_t*>(&bot);
+      }
+      const uint32_t chunk = ((uint32_t)(i % kCpr) + hi) ^ key;
+      stmatrix_x4(lane_row + (uint32_t)(i / kCpr) * kBox + (uint32_t)(8 * j) * kRow + (chunk << 4), h[0], h[1], h[2],
+                  h[3]);
+    }
+  }
+  fence_proxy_async_smem();
+  named_barrier_sync(bar, 128);
+  const int x0 = t.tw * 8 * kS, y0 = t.th * 16 + 8 * g;
+  if (leader) {
+    for (int m = 0; m < kp.st_maps; ++m)
+#pragma unroll
+      for (int b = 0; b < kBN / kBC; ++b) tma_store_4d(&maps.m[m], stage + b * kBox, b * kBC, x0, y0, t.n);
+    bulk_commit_group();
+  }
+  if (pool) {
+    // 16-byte units (8 channels of one pooled pixel) of the 4 x 4S pooled box, read back from the staged tile while
+    // the primary stores read it too; written once those have finished reading.
+    constexpr int kUnits = 2 * kS * kBN, kPer = (kUnits + 127) / 128;
+    auto addr = [&](int pix, int cc, uint32_t box) {
+      const uint32_t k = (((uint32_t)pix * kRow) >> 7) & (uint32_t)(kCpr - 1);
+      return sbase + (uint32_t)(cc / kCpr) * box + (uint32_t)pix * kRow + ((((uint32_t)(cc % kCpr)) ^ k) << 4);
+    };
+    const int tid = threadIdx.x & 127;
+    uint4 pv[kPer];
+#pragma unroll
+    for (int k = 0; k < kPer; ++k) {
+      const int un = tid + 128 * k, cc = un % (kBN / 8), pp = un / (kBN / 8);
+      const int src = (pp / (4 * kS)) * 16 * kS + 2 * (pp % (4 * kS));  // top-left pixel of the 2x2 window
+      if (un < kUnits) {
+        uint4 w[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+          asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
+                       : "=r"(w[e].x), "=r"(w[e].y), "=r"(w[e].z), "=r"(w[e].w)
+                       : "r"(addr(src + (e >> 1) * 8 * kS + (e & 1), cc, kBox))
+                       : "memory");
+        const __half2* h0 = reinterpret_cast<const __half2*>(&w[0]);
+        const __half2* h1 = reinterpret_cast<const __half2*>(&w[1]);
+        const __half2* h2 = reinterpret_cast<const __half2*>(&w[2]);
+        const __half2* h3 = reinterpret_cast<const __half2*>(&w[3]);
+        __half2* o = reinterpret_cast<__half2*>(&pv[k]);
+#pragma unroll
+        for (int c = 0; c < 4; ++c) o[c] = __hmax2(__hmax2(h0[c], h1[c]), __hmax2(h2[c], h3[c]));
+      }
+    }
+    if (leader) bulk_wait_group_read0();
+    named_barrier_sync(bar, 128);
+#pragma unroll
+    for (int k = 0; k < kPer; ++k) {
+      const int un = tid + 128 * k;
+      if (un < kUnits)
+        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr(un / (kBN / 8), un % (kBN / 8), kPoolBox)),
+                     "r"(pv[k].x), "r"(pv[k].y), "r"(pv[k].z), "r"(pv[k].w)
+                     : "memory");
+    }
+    fence_proxy_async_smem();
+    named_barrier_sync(bar, 128);
+    if (leader) {
+#pragma unroll
+      for (int b = 0; b < kBN / kBC; ++b)
+        tma_store_4d(&maps.m[kp.st_maps], stage + b * kPoolBox, b * kBC, x0 >> 1, y0 >> 1, t.n);
+      bulk_commit_group();
+    }
+  }
+}
+
 // kS (sub-tiles), kSteps (16-element k-steps per channel block) and kBN (the N tile = cout_pad) are compile-time so
 // the wgmma issue loop is straight-line code with immediate descriptor offsets, the accumulator array holds exactly
 // the kS * ceil(kBN / 32) * 16 registers this layer needs, and the epilogue indexes it with constants.  One
@@ -39,7 +169,7 @@ __device__ __forceinline__ HaloTile halo_decode(const ConvKParams& kp, int tile)
 template <int kS, int kSteps, int kBN, int kEpi>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
-                 const __grid_constant__ ConvKParams kp) {
+                 const __grid_constant__ ConvKParams kp, const __grid_constant__ HaloStoreMaps tmap_o) {
   constexpr int kNch = (kBN + 31) / 32;  // 32-column epilogue chunks per sub-tile
   constexpr int kAcc = kS * kNch * 16;   // fp32 accumulators per consumer thread
   static_assert(kAcc <= kConvAccRegs, "accumulators of kS sub-tiles must fit the registers");
@@ -47,7 +177,8 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* a_base = smem;
   uint8_t* b_base = smem + (size_t)kp.a_stages * kp.a_bytes;
-  HaloSmemTail* tail = reinterpret_cast<HaloSmemTail*>(b_base + (size_t)kp.b_stages * kp.b_bytes);
+  uint8_t* st_base = b_base + (size_t)kp.b_stages * kp.b_bytes;  // TMA-store staging, kp.st_bytes / 2 per warpgroup
+  HaloSmemTail* tail = reinterpret_cast<HaloSmemTail*>(st_base + kp.st_bytes);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -70,6 +201,7 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     fence_mbar_init();
   }
   if (warp == 1 && lane == 0) tma_prefetch_desc(&tmap_w);
+  if (warp == 2 && lane < kp.st_maps + kp.st_pool) tma_prefetch_desc(&tmap_o.m[lane]);
   for (int i = threadIdx.x; i < kp.cout_pad; i += blockDim.x) tail->bias[i] = kp.bias[i];
   __syncthreads();
   // PDL: the prologue above touched constant data only; from here on activations are read and written.  The weight
@@ -181,6 +313,13 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     wgmma_fence_operands(acc);
     if (!kp.b_resident) consumer_release(&tail->b_empty[prev_b], lane);
     consumer_release(&tail->a_empty[prev_a], lane);
+    if constexpr (kEpi != PB_EPI_SILU_RES) {  // a residual keeps the per-lane store epilogue
+      if (kp.st_bytes != 0) {
+        halo_epilogue_tma<kEpi, kS, kBN>(kp, tmap_o, acc, tail->bias, st_base + (size_t)g * (kp.st_bytes / 2), t, g,
+                                         wq, lane);
+        continue;
+      }
+    }
     const int oh = t.th * 16 + row, ow0 = t.tw * 8 * S + col;
     epilogue_tile<kEpi, kS, kNch>(kp, acc, S, 0, tail->bias, scr, lane, [&](int j, bool& pool_writer) {
       EpiPix px;
@@ -193,9 +332,10 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       return px;
     });
   }
+  if (kp.st_bytes != 0 && (threadIdx.x & 127) == 0) bulk_wait_group0();  // the stores complete before the CTA exits
 }
 
-typedef void (*HaloKernelFn)(CUtensorMap, CUtensorMap, ConvKParams);
+typedef void (*HaloKernelFn)(CUtensorMap, CUtensorMap, ConvKParams, HaloStoreMaps);
 
 // Instantiations: every N tile a halo set-up can produce (cout_pad = 16 .. 256 in steps of 16) with every sub-tile
 // count whose accumulators fit (S * ceil(N / 32) * 16 <= kConvAccRegs), for k-steps 1 / 2 / 4 (KB = 16 / 32 / 64).

@@ -143,6 +143,17 @@ struct ConvKParams {
   int hs_tap_off[9];                                   // smem row offset of each tap's first pixel
   int hs_tap_desc[9];                                  // the same in 16-byte descriptor units (offset * row_bytes / 16)
   int dbg_flags;   // PADEL_B200_CONV_DEBUG: bit0 = plain two-MUFU SiLU (default: one reciprocal per four values), bit1 = no fast epilogue
+  // halo variant, TMA-store epilogue: staging bytes per CTA (0 = per-lane stores), number of output maps the staging
+  // tile is stored through (1 plain, 4 for a 2x2-replicated output, +4 for a PB_OUT2_UP2 copy), 1 = PB_OUT2_POOL2
+  // through map st_maps
+  uint32_t st_bytes;
+  int st_maps, st_pool;
+};
+
+// Output tensor maps of the halo kernel's TMA-store epilogue (ConvKParams::st_maps, st_pool).
+constexpr int kHaloStoreMaps = 5;
+struct HaloStoreMaps {
+  CUtensorMap m[kHaloStoreMaps];
 };
 
 struct ConvPlan {
@@ -150,6 +161,7 @@ struct ConvPlan {
   ConvKParams kp;
   CUtensorMap tmap_a;
   CUtensorMap tmap_w;
+  HaloStoreMaps tmap_o;
   int grid;
   int threads;
   size_t smem_bytes;

@@ -1,4 +1,4 @@
-// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), setmaxnreg, wgmma.
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), stmatrix, setmaxnreg, wgmma.
 // Hand-written for this repo; no CUTLASS/CuTe dependency.
 #pragma once
 #include <cstdint>
@@ -85,6 +85,36 @@ __device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* m, uin
       "%7}], [%2];" ::"r"(smem_u32(dst)),
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
       : "memory");
+}
+
+// ----------------------------------------------------------------------------------------------
+// TMA tiled stores (shared -> global), completion tracked per thread in bulk groups
+// ----------------------------------------------------------------------------------------------
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, const void* src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(m)),
+               "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the shared-memory sources of all committed stores have been read (the staging area may be rewritten)
+__device__ __forceinline__ void bulk_wait_group_read0() {
+  asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+}
+// all committed stores have completed
+__device__ __forceinline__ void bulk_wait_group0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+
+// barrier over `count` threads (a multiple of 32) on hardware barrier `id` (0 is __syncthreads)
+__device__ __forceinline__ void named_barrier_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
+// Four 8x8 fp16 matrices, one 16-byte row per lane address (lane l: row l % 8 of matrix l / 8); register j of every
+// lane holds its two elements of matrix j in the mma fragment layout (row l / 4, columns 2 (l % 4) + {0, 1}).
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1),
+               "r"(r2), "r"(r3)
+               : "memory");
 }
 
 // setmaxnreg: producers give registers back, consumers take them (executed by every warp of the warpgroup)
