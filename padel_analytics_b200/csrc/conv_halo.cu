@@ -44,7 +44,7 @@ static int halo_plan_store(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn 
   kp.st_pool = 0;
   const bool f16 = d->out_mode == PB_OUT_F16_NHWC || d->out_mode == PB_OUT_F16_NHWC_UP2;
   if (!enabled || kp.dbg_flags != 0 || d->res || d->head_n != 0 || !f16 || plan->epi == PB_EPI_SILU_RES ||
-      d->cout_store != kp.BN || ((d->out_C | d->out_coff) & 7) != 0)
+      d->cout_store != kp.n_ntiles * kp.BN || ((d->out_C | d->out_coff) & 7) != 0)
     return 0;
   // Deep-K streamed layers (more than two channel blocks) are mainloop-bound and need their third halo stage and
   // deep weight ring more than an asynchronous epilogue (H100: up_block_2.conv_1 of TrackNet ran 5 % slower with it).
@@ -58,7 +58,8 @@ static int halo_plan_store(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn 
     else if (!kp.b_resident && bs > 3) --bs;
     else return 0;
   }
-  // one map per destination of the staging box (channels, 8S columns, 8 rows, image); base = channel 0 of the slice
+  // one map per destination of the staging box (channels, 8S columns, 8 rows, image); base = channel 0 of the slice,
+  // which spans the N tiles' cout_store channels
   const int S = kp.hs_S, bc = halo_store_box_channels(kp.BN);
   const CUtensorMapSwizzle swz = bc == 64 ? CU_TENSOR_MAP_SWIZZLE_128B
                                  : bc == 32 ? CU_TENSOR_MAP_SWIZZLE_64B
@@ -67,7 +68,7 @@ static int halo_plan_store(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn 
   auto add = [&](void* out, int C, int coff, int W, int H, int up, int dy, int dx, int bw, int bh) {
     const size_t pxb = (size_t)C * 2;
     char* base = reinterpret_cast<char*>(out) + ((size_t)(dy * up * W + dx) * C + coff) * 2;
-    cuuint64_t dims[4] = {(cuuint64_t)kp.BN, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)kp.N};
+    cuuint64_t dims[4] = {(cuuint64_t)d->cout_store, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)kp.N};
     cuuint64_t strides[3] = {up * pxb, (cuuint64_t)up * up * W * pxb, (cuuint64_t)up * up * W * H * pxb};
     cuuint32_t box[4] = {(cuuint32_t)bc, (cuuint32_t)bw, (cuuint32_t)bh, 1};
     cuuint32_t estr[4] = {1, 1, 1, 1};
@@ -201,10 +202,19 @@ int conv_stem_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode)
   return 0;
 }
 
-int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode) {
-  if (d->ksize != 3 || d->stride != 1 || d->cout_pad > 256) return -1;
+// cout > 192 runs in N tiles of BN = 128 with streamed weights.  At S = 2 a CTA fetches one 18 x 18-pixel halo and
+// 9 x 128 weight rows per channel block: ~0.010 bytes from L2 per MAC, against 0.023 for the per-tap kernel's
+// 128 x 256 tiles and 0.017 for one S = 1, BN = 256 tile here.  S = 4 / BN = 64 would move fewer bytes still, but an
+// m64n64k16 wgmma reads 4 KB of shared memory per 32 tensor clocks, the SM's whole 128 B/clk, which is why the
+// 64-channel layers trail; BN stays at 128.  Without `force` such a layer is taken only when the 16 x 8S tiles compute
+// at most 1.15x its output pixels (after the rows a warpgroup skips below the image): the per-tap kernel's flattened
+// 128-pixel tiles waste nothing at the edges.  `force`: wherever the kernel can run the layer.
+int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode, bool force) {
+  if (d->ksize != 3 || d->stride != 1) return -1;
+  const bool ntiled = d->cout_pad > 192 && d->cout_pad % kHaloNTileBN == 0 && d->head_n == 0;
+  if (!ntiled && d->cout_pad > (force ? 256 : 192)) return -1;
   ConvKParams& kp = plan->kp;  // common fields (epilogue, KB, kblocks, ...) already filled by the caller
-  const int BN = d->cout_pad;
+  const int BN = ntiled ? kHaloNTileBN : d->cout_pad;
   const uint32_t row_bytes = (uint32_t)kp.KB * 2u;
   const int acc_cols = (BN + 31) / 32 * 32;
   const size_t budget = kHaloSmemBudget;
@@ -219,7 +229,7 @@ int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode)
   bool resident = false;
   {
     const char* er = getenv("PADEL_B200_CONV_BRES");
-    resident = (!er || atoi(er) != 0) && kp.kblocks <= kHaloMaxB && res_total <= 120 * 1024;
+    resident = (!er || atoi(er) != 0) && !ntiled && kp.kblocks <= kHaloMaxB && res_total <= 120 * 1024;
   }
   int bestS = 0, best_cols = 0, G = 1;
   for (int pass = resident ? 0 : 1; pass < 2 && bestS == 0; ++pass) {
@@ -254,6 +264,10 @@ int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode)
   const uint32_t b_alloc = ((uint32_t)G * tap_bytes + 1023u) & ~1023u;
   if (bestS == 0) return -1;
   const int S = bestS, P = 8 * S + 2;
+  if (ntiled && !force) {
+    const long computed = (long)best_cols * ((kp.Ho + 7) / 8 * 8);
+    if (20 * computed > 23 * (long)kp.Wo * kp.Ho) return -1;
+  }
   kp.b_resident = resident ? 1 : 0;
   kp.hs_S = S;
   kp.hs_P = P;
@@ -268,7 +282,7 @@ int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode)
       kp.hs_tap_desc[r * 3 + q] = (int)(((uint32_t)(r * P + q) * row_bytes) >> 4);
     }
   kp.BN = BN;
-  kp.n_ntiles = 1;
+  kp.n_ntiles = d->cout_pad / BN;
   kp.halo_bytes = 18u * (uint32_t)P * row_bytes;
   kp.hs_a_row_bytes = row_bytes;
   kp.a_bytes = (kp.halo_bytes + 1023u) & ~1023u;
@@ -297,7 +311,7 @@ int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode)
   kp.tiles_w = (kp.Wo + 8 * S - 1) / (8 * S);
   kp.tiles_h = (kp.Ho + 15) / 16;
   kp.tiles_n = kp.N;
-  kp.total_tiles = kp.tiles_w * kp.tiles_h * kp.tiles_n;
+  kp.total_tiles = kp.tiles_w * kp.tiles_h * kp.tiles_n * kp.n_ntiles;
   if (halo_plan_store(d, plan, encode) != 0) return 1;
   halo_finish_config(plan);
   plan->variant = 1;

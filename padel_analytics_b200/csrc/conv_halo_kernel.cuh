@@ -10,6 +10,10 @@ namespace pb {
 
 constexpr int kHaloMaxA = 4;
 constexpr int kHaloMaxB = 12;
+// N tile of the layers conv_halo_setup splits into N tiles (cout > 192).  Only the kBN == kHaloNTileBN instantiations
+// carry the N-tile index; in all others it is the constant 0, which keeps the widest ones (S = 1, N = 240: 128
+// accumulators) free of spills.
+constexpr int kHaloNTileBN = 128;
 
 struct HaloSmemTail {
   uint64_t a_full[kHaloMaxA];
@@ -21,12 +25,15 @@ struct HaloSmemTail {
 };
 
 struct HaloTile {
-  int tw, th, n;
+  int nt, tw, th, n;
 };
+// The N tile is the fastest index: the CTAs computing the N tiles of one spatial tile run at the same time, so all but
+// the first read of its halo hit L2.
 __device__ __forceinline__ HaloTile halo_decode(const ConvKParams& kp, int tile) {
   HaloTile t;
   int q;
-  fast_divmod(q, t.tw, tile, kp.fd_w);
+  fast_divmod(q, t.nt, tile, kp.fd_nt);
+  fast_divmod(q, t.tw, q, kp.fd_w);
   fast_divmod(t.n, t.th, q, kp.fd_h);
   return t;
 }
@@ -106,7 +113,8 @@ __device__ __forceinline__ void halo_epilogue_tma(const ConvKParams& kp, const H
   if (leader) {
     for (int m = 0; m < kp.st_maps; ++m)
 #pragma unroll
-      for (int b = 0; b < kBN / kBC; ++b) tma_store_4d(&maps.m[m], stage + b * kBox, b * kBC, x0, y0, t.n);
+      for (int b = 0; b < kBN / kBC; ++b)
+        tma_store_4d(&maps.m[m], stage + b * kBox, t.nt * kBN + b * kBC, x0, y0, t.n);
     bulk_commit_group();
   }
   if (pool) {
@@ -155,7 +163,7 @@ __device__ __forceinline__ void halo_epilogue_tma(const ConvKParams& kp, const H
     if (leader) {
 #pragma unroll
       for (int b = 0; b < kBN / kBC; ++b)
-        tma_store_4d(&maps.m[kp.st_maps], stage + b * kPoolBox, b * kBC, x0 >> 1, y0 >> 1, t.n);
+        tma_store_4d(&maps.m[kp.st_maps], stage + b * kPoolBox, t.nt * kBN + b * kBC, x0 >> 1, y0 >> 1, t.n);
       bulk_commit_group();
     }
   }
@@ -236,11 +244,12 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       int st = 0;
       uint32_t ph = 0;
       for (int tile = blockIdx.x; tile < kp.total_tiles; tile += gridDim.x) {
+        const int co = kBN == kHaloNTileBN ? halo_decode(kp, tile).nt * kBN : 0;  // first channel of the N tile
         for (int cb = 0; cb < kp.kblocks; ++cb) {
           for (int tg = 0; tg < tap_groups; ++tg) {
             if (!kp.b_resident) mbar_wait(&tail->b_empty[st], ph ^ 1);
             mbar_arrive_expect_tx(&tail->b_full[st], kp.b_tx_bytes);
-            tma_load_3d(b_base + (size_t)st * kp.b_bytes, &tmap_w, &tail->b_full[st], cb * kp.KB, 0, tg * G);
+            tma_load_3d(b_base + (size_t)st * kp.b_bytes, &tmap_w, &tail->b_full[st], cb * kp.KB, co, tg * G);
             if (++st == kp.b_stages) {
               st = 0;
               ph ^= 1;
@@ -258,6 +267,9 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   // image rows 8g .. 8g + 7, i.e. the 8-row groups 8g .. 8g + 7 of every tap's A descriptor.
   warpgroup_reg_alloc<kConvConsumerRegs>();
   const int cw = warp - 4, g = cw >> 2, wq = cw & 3;
+  // g broadcast from lane 0: the compiler then knows the warpgroup skip test below, and with it the ring positions
+  // after it, are warp-uniform, and keeps the descriptor arithmetic in uniform registers
+  const int g_uni = __shfl_sync(0xffffffffu, g, 0);
   float* scr = tail->scratch + cw * kEpiScratchFloats;
   const uint32_t sbo = (uint32_t)kp.hs_sbo_rows * a_row_bytes;
   const uint64_t g_units = (uint64_t)((8u * (uint32_t)g * sbo) >> 4);
@@ -271,7 +283,30 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   int ast = 0, bst = 0;
   uint32_t aph = 0, bph = 0;
   for (int tile = blockIdx.x; tile < kp.total_tiles; tile += gridDim.x) {
-    const HaloTile t = halo_decode(kp, tile);
+    HaloTile t = halo_decode(kp, tile);
+    if constexpr (kBN != kHaloNTileBN) t.nt = 0;
+    if (t.th * 16 + 8 * g_uni >= kp.Ho) {
+      // All 8 image rows of this warpgroup lie below the image (last tile row of a height that is not a multiple of
+      // 16): no wgmmas and no stores.  It still waits on every stage and releases it -- the empty barriers count its
+      // warps' arrivals -- and keeps the ring phases in step with its partner.
+      for (int cb = 0; cb < kp.kblocks; ++cb) {
+        mbar_wait(&tail->a_full[ast], aph);
+        for (int tg = 0; tg < tap_groups; ++tg) {
+          mbar_wait(&tail->b_full[bst], kp.b_resident ? 0u : bph);
+          if (!kp.b_resident) consumer_release(&tail->b_empty[bst], lane);
+          if (++bst == kp.b_stages) {
+            bst = 0;
+            bph ^= 1;
+          }
+        }
+        consumer_release(&tail->a_empty[ast], lane);
+        if (++ast == kp.a_stages) {
+          ast = 0;
+          aph ^= 1;
+        }
+      }
+      continue;
+    }
     // One group of wgmmas (one weight stage) stays in flight while the next is issued: a weight stage is released
     // once the group after it has been issued and wgmma_wait<1> has retired it, a halo stage once the first group
     // of the next channel block has (prev_b / prev_a: the stages still read by the group in flight, -1 = none).
@@ -313,15 +348,16 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     wgmma_fence_operands(acc);
     if (!kp.b_resident) consumer_release(&tail->b_empty[prev_b], lane);
     consumer_release(&tail->a_empty[prev_a], lane);
+    const float* sbias = tail->bias + t.nt * kBN;
     if constexpr (kEpi != PB_EPI_SILU_RES) {  // a residual keeps the per-lane store epilogue
       if (kp.st_bytes != 0) {
-        halo_epilogue_tma<kEpi, kS, kBN>(kp, tmap_o, acc, tail->bias, st_base + (size_t)g * (kp.st_bytes / 2), t, g,
-                                         wq, lane);
+        halo_epilogue_tma<kEpi, kS, kBN>(kp, tmap_o, acc, sbias, st_base + (size_t)g * (kp.st_bytes / 2), t, g, wq,
+                                         lane);
         continue;
       }
     }
     const int oh = t.th * 16 + row, ow0 = t.tw * 8 * S + col;
-    epilogue_tile<kEpi, kS, kNch>(kp, acc, S, 0, tail->bias, scr, lane, [&](int j, bool& pool_writer) {
+    epilogue_tile<kEpi, kS, kNch>(kp, acc, S, t.nt, sbias, scr, lane, [&](int j, bool& pool_writer) {
       EpiPix px;
       px.n = t.n;
       px.oh = oh;

@@ -318,18 +318,21 @@ static int conv_plan_build_impl(const pb_conv_desc* d, ConvPlan* plan) {
   plan->epi = conv_epi_class(d, kp);
   if (stem) return conv_stem_setup(d, plan, encode);
   {
-    // halo variant for 3x3/s1 layers: default on for cout <= 192 (the layers the per-tap kernel leaves
-    // L2/TMA-bound); PADEL_B200_CONV_HALO=0 disables it, =1 forces it wherever it applies
+    // halo variant: default on for cout <= 192 (the layers the per-tap kernel leaves L2/TMA-bound) and for the 3x3 / s1
+    // layers conv_halo_setup runs in N tiles with little edge waste; PADEL_B200_CONV_HALO=0 disables it, =1 forces it
+    // wherever it applies.  PB_OUT2_POOL2 exists in the halo kernel only, so such a layer takes it wherever it can.
     const char* e = getenv("PADEL_B200_CONV_HALO");
     const int mode = e ? atoi(e) : 2;
-    if (mode == 1 || (mode == 2 && d->cout_pad <= 192)) {
+    const bool s1_3x3 = d->ksize == 3 && d->stride == 1;
+    if (mode == 1 || (mode == 2 && (d->cout_pad <= 192 || s1_3x3))) {
       const int rc = d->ksize == 1    ? conv_halo_1x1_setup(d, plan, encode)
                      : d->stride == 2 ? conv_halo_s2_setup(d, plan, encode)
-                                      : conv_halo_setup(d, plan, encode);
+                                      : conv_halo_setup(d, plan, encode, mode == 1 || d->out2_mode == PB_OUT2_POOL2);
       if (rc >= 0) return rc;
     }
   }
-  PB_CHECK(d->out2_mode != PB_OUT2_POOL2, "conv: PB_OUT2_POOL2 is only implemented by the halo kernel (cout <= 192)");
+  PB_CHECK(d->out2_mode != PB_OUT2_POOL2,
+           "conv: PB_OUT2_POOL2 is only implemented by the halo kernel (3x3 stride 1, cout <= 256 or a multiple of 128)");
   // N tile: largest multiple-of-16 divisor of cout_pad that is <= 256
   int nn = (d->cout_pad + 255) / 256;
   while (d->cout_pad % nn != 0 || (d->cout_pad / nn) % 16 != 0) ++nn;

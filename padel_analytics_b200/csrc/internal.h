@@ -181,7 +181,7 @@ int conv_epi_class(const pb_conv_desc* d, const ConvKParams& kp);
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode);  // -1: not applicable
+int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode, bool force);  // -1: not applicable
 int conv_stem_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode);
 int conv_halo_s2_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode);  // -1: not applicable
 int conv_halo_1x1_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode);  // -1: not applicable

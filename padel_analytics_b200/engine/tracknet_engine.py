@@ -116,7 +116,7 @@ class TrackNetEngine:
                                       out2=None if pool is None else (pool, 0, L.OUT2_POOL2)),
                    cin_real=27 if name == "down_block_1.conv_1" else cin)
 
-        # MaxPool2d of the first two encoder blocks (models.py:60,62) is a second store of the producing conv
+        # MaxPool2d of the three encoder blocks (models.py:60,62,64) is a second store of the producing conv
         # (PB_OUT2_POOL2); PADEL_B200_FUSE_OUT2=0 keeps the separate pool launches (A/B)
         fuse = os.environ.get("PADEL_B200_FUSE_OUT2", "1") != "0"
 
@@ -130,8 +130,9 @@ class TrackNetEngine:
             P.maxpool2(self.cat2, 256, 128, self.p2, 0)
         conv(self.p2, 0, 128, "down_block_3.conv_1", self.t3a, 0)
         conv(self.t3a, 0, 256, "down_block_3.conv_2", self.t3b, 0)
-        conv(self.t3b, 0, 256, "down_block_3.conv_3", self.cat1, 512)
-        P.maxpool2(self.cat1, 512, 256, self.p3, 0)
+        conv(self.t3b, 0, 256, "down_block_3.conv_3", self.cat1, 512, pool=self.p3 if fuse else None)
+        if not fuse:
+            P.maxpool2(self.cat1, 512, 256, self.p3, 0)
         conv(self.p3, 0, 256, "bottleneck.conv_1", self.ba, 0)
         conv(self.ba, 0, 512, "bottleneck.conv_2", self.bb, 0)
         conv(self.bb, 0, 512, "bottleneck.conv_3", self.cat1, 0, UP)  # nearest x2 fused into the store
