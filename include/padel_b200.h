@@ -126,6 +126,37 @@ int pb_program_num_ops(const pb_program* p);
 /* Kernel that op i launches: 0 conv_tc_kernel (per-tap boxes), 1 conv_halo_kernel (shared halo / stem), 2 maxpool2,
  * 3 upsample2, 4 sppf_pool, 5 pointwise_head; -1 if i is out of range. */
 int pb_program_op_kernel(const pb_program* p, int i);
+/* What op i of a program runs, for tests and tools (introspection only: no plan depends on it). */
+#define PB_CONV_PER_TAP 0   /* conv_tc_kernel                                  */
+#define PB_CONV_HALO 1      /* conv_halo_kernel, 3x3 stride 1                 */
+#define PB_CONV_HALO_1X1 2  /* conv_halo_kernel, 1x1 stride 1                 */
+#define PB_CONV_HALO_S2 3   /* conv_halo_kernel, 3x3 stride 2 pixel-pair view */
+#define PB_CONV_STEM 4      /* conv_halo_kernel, PB_IN_STEM4 input            */
+typedef struct pb_op_info {
+  int kernel; /* as pb_program_op_kernel */
+  /* conv ops (kernel 0 / 1): the plan */
+  int variant;              /* PB_CONV_*                                                                      */
+  int epi;                  /* epilogue class: 0 run-time, 1 SiLU, 2 ReLU, 3 SiLU + residual, 4 fp32 NHWC     */
+  int S, G, BN, n_ntiles;   /* sub-tiles per CTA tile, taps per weight box (halo), N tile, N tiles            */
+  int KB, kblocks;          /* channels per K block, K blocks                                                 */
+  int b_resident;           /* halo: the whole filter bank stays in shared memory                             */
+  int a_stages, b_stages;   /* halo: activation / weight ring depths                                         */
+  int tma_store, st_pool;   /* halo: fp16 outputs through the TMA-store staging tile, pooled second store too */
+  /* The per-tap kernel has no halo fields of its own: it reports S = G = 1 (one 128-pixel tile, one tap per box),
+   * b_resident = tma_store = st_pool = 0, and its single ring of combined activation + weight stages as
+   * a_stages = b_stages.  Tools that compare halo plans should select variant != PB_CONV_PER_TAP first.         */
+  int grid, total_tiles, pdl;
+  pb_conv_desc desc;        /* the descriptor the plan was built from                                        */
+  /* maxpool2 / upsample2 / sppf / pointwise head (kernel 2..5): the arguments they were added with; sppf: in == out
+   * = the concat buffer, c = its slice width; pointwise head: c = n_out, weight / bias = its parameters          */
+  const void* in;
+  void* out;
+  int N, H, W, C, c_off, c, out_C, out_coff;
+  const float* weight;
+  const float* bias;
+} pb_op_info;
+/* Fills *out for op i; returns non-zero if i is out of range. */
+int pb_program_op_info(const pb_program* p, int i, pb_op_info* out);
 int pb_program_run(pb_program* p, void* stream);
 /* Run ops [first, last) only (per-layer timing / debugging). */
 int pb_program_run_range(pb_program* p, int first, int last, void* stream);

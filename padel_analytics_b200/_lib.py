@@ -35,6 +35,24 @@ class ConvDesc(C.Structure):
     ]
 
 
+class OpInfo(C.Structure):
+    """pb_op_info: what one op of a program runs (pb_program_op_info)."""
+    _fields_ = [
+        ("kernel", C.c_int),
+        ("variant", C.c_int), ("epi", C.c_int),
+        ("S", C.c_int), ("G", C.c_int), ("BN", C.c_int), ("n_ntiles", C.c_int),
+        ("KB", C.c_int), ("kblocks", C.c_int),
+        ("b_resident", C.c_int), ("a_stages", C.c_int), ("b_stages", C.c_int),
+        ("tma_store", C.c_int), ("st_pool", C.c_int),
+        ("grid", C.c_int), ("total_tiles", C.c_int), ("pdl", C.c_int),
+        ("desc", ConvDesc),
+        ("in_", C.c_void_p), ("out", C.c_void_p),
+        ("N", C.c_int), ("H", C.c_int), ("W", C.c_int), ("C", C.c_int),
+        ("c_off", C.c_int), ("c", C.c_int), ("out_C", C.c_int), ("out_coff", C.c_int),
+        ("weight", C.c_void_p), ("bias", C.c_void_p),
+    ]
+
+
 class YoloLevel(C.Structure):
     _fields_ = [("feat", C.c_void_p), ("h", C.c_int), ("w", C.c_int), ("stride", C.c_int)]
 
@@ -43,6 +61,7 @@ ACT_NONE, ACT_RELU, ACT_SILU, ACT_SIGMOID = 0, 1, 2, 3
 OUT_F16_NHWC, OUT_F16_NHWC_UP2, OUT_F32_NHWC, OUT_F32_NCHW, OUT_NONE = 0, 1, 2, 3, 4
 IN_NHWC, IN_STEM4 = 0, 1
 OUT2_NONE, OUT2_UP2, OUT2_POOL2 = 0, 1, 2
+CONV_PER_TAP, CONV_HALO, CONV_HALO_1X1, CONV_HALO_S2, CONV_STEM = 0, 1, 2, 3, 4
 
 # name -> (restype, argtypes); must list every symbol of include/padel_b200.h (tests check this)
 _i, _p, _f = C.c_int, C.c_void_p, C.c_float
@@ -61,6 +80,7 @@ SIGNATURES = {
     "pb_program_add_pointwise_head": (_i, [_p, _p, _i, _i, _i, _i, _p, _p, _i, _p]),
     "pb_program_num_ops": (_i, [_p]),
     "pb_program_op_kernel": (_i, [_p, _i]),
+    "pb_program_op_info": (_i, [_p, _i, C.POINTER(OpInfo)]),
     "pb_program_run": (_i, [_p, _p]),
     "pb_program_run_range": (_i, [_p, _i, _i, _p]),
     "pb_letterbox_u8_f16": (_i, [_p, _i, _i, _i, _p, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p, _i, _i, _i, _i, _p]),

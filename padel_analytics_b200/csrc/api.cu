@@ -1,5 +1,6 @@
 // C-ABI surface of libpadel_b200.so: error reporting, programs (op lists), one-shot conv launches.
 #include <atomic>
+#include <cstring>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -171,6 +172,60 @@ int pb_program_op_kernel(const pb_program* p, int i) {
     case OpKind::PointwiseHead: return 5;
   }
   return -1;
+}
+
+int pb_program_op_info(const pb_program* p, int i, pb_op_info* out) {
+  PB_CHECK(p && out, "program_op_info: null argument");
+  PB_CHECK(i >= 0 && i < (int)p->ops.size(), "program_op_info: op %d out of range", i);
+  const Op& op = p->ops[i];
+  memset(out, 0, sizeof(*out));
+  out->kernel = pb_program_op_kernel(p, i);
+  if (op.kind == OpKind::Conv) {
+    const ConvPlan& pl = *op.conv;
+    const ConvKParams& kp = pl.kp;
+    const pb_conv_desc& d = pl.desc;
+    out->desc = d;
+    out->variant = pl.variant != 1                ? PB_CONV_PER_TAP
+                   : d.in_layout == PB_IN_STEM4   ? PB_CONV_STEM
+                   : d.ksize == 1                 ? PB_CONV_HALO_1X1
+                   : d.stride == 2                ? PB_CONV_HALO_S2
+                                                  : PB_CONV_HALO;
+    out->epi = pl.epi;
+    out->BN = kp.BN;
+    out->n_ntiles = kp.n_ntiles;
+    out->KB = kp.KB;
+    out->kblocks = kp.kblocks;
+    if (pl.variant == 1) {
+      out->S = kp.hs_S;
+      out->G = kp.hs_G;
+      out->b_resident = kp.b_resident;
+      out->a_stages = kp.a_stages;
+      out->b_stages = kp.b_stages;
+      out->tma_store = kp.st_bytes != 0;
+      out->st_pool = kp.st_pool;
+    } else {
+      out->S = 1;
+      out->G = 1;
+      out->a_stages = out->b_stages = kp.stages;
+    }
+    out->grid = pl.grid;
+    out->total_tiles = kp.total_tiles;
+    out->pdl = pl.pdl;
+  } else {
+    out->in = op.in;
+    out->out = op.out;
+    out->N = op.N;
+    out->H = op.H;
+    out->W = op.W;
+    out->C = op.C;
+    out->c_off = op.c_off;
+    out->c = op.c;
+    out->out_C = op.out_C;
+    out->out_coff = op.out_coff;
+    out->weight = op.hw;
+    out->bias = op.hb;
+  }
+  return 0;
 }
 
 int pb_program_run_range(pb_program* p, int first, int last, void* stream) {

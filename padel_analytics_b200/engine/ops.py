@@ -194,6 +194,13 @@ class Program:
                  4: "sppf_pool_kernel", 5: "pointwise_head_kernel"}
         return [names[L.lib().pb_program_op_kernel(self._h, i)] for i in range(self.num_ops)]
 
+    def op_info(self, i: int) -> L.OpInfo:
+        """The plan of conv op i (variant, epilogue class, S, G, N tiles, rings, TMA store, grid, ...) and its
+        descriptor, or the pointers and dims of any other op (pb_program_op_info)."""
+        info = L.OpInfo()
+        L.check(L.lib().pb_program_op_info(self._h, i, C.byref(info)))
+        return info
+
     def run(self, first: int | None = None, last: int | None = None):
         if first is None:
             L.check(L.lib().pb_program_run(self._h, L.stream_ptr()))
