@@ -270,6 +270,24 @@ int pb_tracknet_ensemble(const float* pred, int S, int first_window, int total_w
  * bbox: int (nframes,4) = x,y,w,h (0,0,0,0 if empty). scratch: int32 (nframes, 5, H*W).                          */
 int pb_ccl_bbox(const uint8_t* mask, int nframes, int H, int W, int* scratch, int* bbox, void* stream);
 
+/* ---- Render pass overlay compositor (runner.py:91-173: tracker drawings, mini-court, projections) --------------- */
+/* One display-list record.  The rectangle (x0, y0, w, h) is in frame pixels; the part outside the frame is skipped.
+ * STAMP: every pixel whose coverage byte atlas[atlas_offset + (y - y0) * pitch + (x - x0)] is non-zero becomes
+ *        colour_bgr (byte 0 = B, 1 = G, 2 = R).
+ * BLEND: every byte v of the rectangle becomes blend_lut[v].                                                      */
+enum { PB_OVERLAY_STAMP = 0, PB_OVERLAY_BLEND = 1 };
+typedef struct pb_overlay_rec {
+  int x0, y0, w, h;
+  int atlas_offset, pitch;
+  uint32_t colour_bgr;
+  int op;
+} pb_overlay_rec;
+/* In place on frames u8 (B,H,W,3) BGR (device).  list (device) holds frame f's records at
+ * [list_offsets[f], list_offsets[f+1]) in draw order; list_offsets int (B+1) (device); atlas u8 (device) the
+ * coverage sprites; blend_lut u8 (256) (device).  Overlapping records resolve in draw order.                      */
+int pb_render_overlay(uint8_t* frames, int B, int H, int W, const pb_overlay_rec* list, const int* list_offsets,
+                      const uint8_t* atlas, const uint8_t* blend_lut, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

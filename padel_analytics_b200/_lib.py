@@ -105,7 +105,13 @@ SIGNATURES = {
     "pb_median_u8": (_i, [_p, _i, C.c_longlong, _p, _i, _p]),
     "pb_tracknet_ensemble": (_i, [_p, _i, _i, _i, _i, _i, _i, _i, _f, _p, _p, _p]),
     "pb_ccl_bbox": (_i, [_p, _i, _i, _i, _p, _p, _p]),
+    "pb_render_overlay": (_i, [_p, _i, _i, _i, _p, _p, _p, _p, _p]),
 }
+
+OVERLAY_STAMP, OVERLAY_BLEND = 0, 1
+# pb_overlay_rec as a numpy structured dtype (32 bytes, the C layout): display lists are built as numpy arrays
+OVERLAY_REC = [("x0", "<i4"), ("y0", "<i4"), ("w", "<i4"), ("h", "<i4"), ("atlas_offset", "<i4"), ("pitch", "<i4"),
+               ("colour_bgr", "<u4"), ("op", "<i4")]
 
 _lib = None
 

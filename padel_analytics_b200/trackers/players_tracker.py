@@ -90,6 +90,17 @@ class Player:
                     (0, 200, 255), 1)
         return frame
 
+    def draw_projection(self, frame):
+        """The player on the mini court (players_tracker.py:171-190): a filled circle at `projection` and the id."""
+        import cv2
+
+        if not self.projection:
+            raise ValueError("Inexistent projection.")
+        cv2.circle(frame, self.projection, 8, (0, 0, 255), -1)
+        cv2.putText(frame, str(self.id), (self.projection[0], self.projection[1] - 10), cv2.FONT_HERSHEY_SIMPLEX, 0.9,
+                    (0, 0, 255), 2)
+        return frame
+
 
 class Players(Object):
     """All tracked players of one frame (players_tracker.py:199-263).  Array-backed like PlayersKeypoints: the tracker

@@ -1,7 +1,16 @@
 """TrackingRunner: the per-tracker pass over a video (API of /root/reference/trackers/runner.py:37-236), plus the
 multi-GPU sharded variant (SURVEY §8e): one process per GPU, contiguous frame ranges, no per-batch collectives —
 detections are gathered once per tracker and the sequential host stages (ByteTrack ids, JSON) run on rank 0.
-The drawing / data-collection pass (runner.py:91-173) is outside the hot path and is not reproduced.
+
+After the trackers, `run()` renders the annotated video to `inference_path` and collects the players' court positions
+into `data_analytics` (runner.py:91-173) when either is asked for; the overlays are composited on the device
+(render.py, `pb_render_overlay`) and encoding runs on a thread of its own.
+
+Documented deviations from reference quirks (SURVEY App. E):
+  q7  with collect_data=False the reference's drawing pass ends by trimming `self.data_analytics.frames`, which is
+      None, and raises AttributeError; here the trim happens only when data is collected.
+  No per-frame prints; `data_analytics` is also filled when no video is written (collect_data=True without an
+  inference_path), without rendering any frame.
 """
 from __future__ import annotations
 
@@ -15,10 +24,11 @@ import torch
 from . import sv_compat as sv
 from ..engine.yolo_engine import ResultBlock
 from .ball_tracker import Ball, BallTracker
-from .keypoints_tracker import KeypointsTracker
+from .keypoints_tracker import Keypoints, KeypointsTracker
 from .players_keypoints_tracker import PlayerKeypointsTracker
-from .players_tracker import PlayerTracker
+from .players_tracker import PlayerTracker, Players
 from .tracker import Tracker, sampler
+from ..analytics import DataAnalytics, ProjectedCourt
 
 
 def shard_range(total: int, rank: int, world: int) -> tuple[int, int]:
@@ -187,11 +197,21 @@ class TrackingRunner:
             self.total_frames = (total if end is None else min(end, total)) - start if total is not None else None
             for t in self.trackers.values():
                 t.video_info_post_init(video_info)  # runner.py:61-62
+        # runner.py:59-79: fixed court keypoints keep the first homography; the mini court needs the frame size
+        self.is_fixed_keypoints = any(getattr(t, "fixed_keypoints_detection", None) is not None
+                                      for t in self.trackers.values() if isinstance(t, KeypointsTracker))
+        self.collect_data = collect_data
+        self.projected_court = ProjectedCourt(video_info) if video_info is not None else None
+        self.data_analytics = DataAnalytics() if collect_data else None
+        self.render_batch_size = 32
+        self._source = None  # (frame_source, total_frames) of the last run(), for the drawing pass
         self.timings: dict[str, float] = {}
 
     def restart(self) -> None:
         for t in self.trackers.values():
             t.restart()
+        if self.data_analytics:
+            self.data_analytics.restart()
 
     def _frames(self, lo: int, hi: int) -> Iterable[np.ndarray]:
         return sv.get_video_frames_generator(self.video_path, start=self.start + lo, end=self.start + hi)
@@ -217,16 +237,25 @@ class TrackingRunner:
         gc_was_on = gc.isenabled()
         gc.disable()
         try:
-            return self._run(frame_source, total_frames, fused)
+            timings = self._run(frame_source, total_frames, fused)
         finally:
             if gc_was_on:
                 gc.enable()
+        import torch.distributed as dist
+
+        rank = dist.get_rank() if dist.is_available() and dist.is_initialized() else 0
+        if rank == 0 and (self.inference_path or self.data_analytics is not None):  # rank 0 holds every result
+            t0 = timeit.default_timer()
+            self.draw_and_collect_data()
+            timings["_render"] = timeit.default_timer() - t0
+        return timings
 
     def _run(self, frame_source, total_frames, fused) -> dict[str, float]:
         import torch.distributed as dist
 
         src = frame_source or self._frames
         total = total_frames if total_frames is not None else self.total_frames
+        self._source = (src, total)
         dist_on = dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1
         rank, world = (dist.get_rank(), dist.get_world_size()) if dist_on else (0, 1)
         lo, hi = shard_range(total, rank, world)
@@ -263,6 +292,92 @@ class TrackingRunner:
             if rank == 0:
                 tracker.save_predictions()
         return self.timings
+
+    # ---- drawing pass (runner.py:91-173) -----------------------------------------------------------------------
+    def _render_source(self, frame_source):
+        if frame_source is not None:
+            return frame_source, len(next(iter(self.trackers.values())).results)
+        if self._source is not None:
+            return self._source
+        return self._frames, self.total_frames
+
+    def _render_batches(self, frame_source, data_analytics, free_slots=None, renderer=None):
+        """(renderer, iterator over (frames, out_slot) batches) of the whole video, overlays composited."""
+        from ..render import DisplayListBuilder, OverlayRenderer, frame_batches
+
+        if self.projected_court is None:
+            raise ValueError("rendering needs video_info (the frame size of the mini court)")
+        src, total = self._render_source(frame_source)
+        self.projected_court.H = None  # every pass starts from the first frame's keypoints
+        hw = (self.video_info.height, self.video_info.width)
+        builder = DisplayListBuilder(hw, self.projected_court)
+        if renderer is None:
+            renderer = OverlayRenderer(hw, self.render_batch_size, builder.lut,
+                                       out_slots=3 if free_slots is not None else 2)
+
+        def build(first, n):
+            return [builder.frame_records(first + j, self.trackers, data_analytics, self.is_fixed_keypoints)
+                    for j in range(n)]
+
+        def checked(batches):
+            for b in batches:
+                if tuple(b[0].shape[:2]) != hw:
+                    raise ValueError(f"frames are {tuple(b[0].shape[:2])}, video_info says {hw}")
+                yield b
+
+        return renderer, renderer.run(checked(frame_batches(src(0, total), self.render_batch_size)), build, free_slots)
+
+    def render_frames(self, frame_source: Optional[Callable[[int, int], Iterable[np.ndarray]]] = None,
+                      data_analytics: Optional[DataAnalytics] = None) -> Iterable[np.ndarray]:
+        """The run's frames with the drawings of runner.py:114-162 (frame number, every tracker's `draw`, mini
+        court, projected players and ball), as uint8 BGR host frames, one per video frame.  `frame_source` is the
+        callable `run()` takes (default: the one the last `run()` used, else the video).  Positions go to
+        `data_analytics` when one is given.  The overlays are composited on the device in batches."""
+        _, batches = self._render_batches(frame_source, data_analytics)
+        for frames, _ in batches:
+            for f in frames:
+                yield f.copy()
+
+    def draw_and_collect_data(self, frame_source=None) -> None:
+        """runner.py:91-173: writes the rendered video to `inference_path` (cv2.VideoWriter, mp4v, the video's fps and
+        size; encoding on a writer thread, overlapping the next batch) and fills `data_analytics` when collecting."""
+        import queue
+
+        from ..render import VideoWriterThread
+
+        if self.data_analytics is not None:
+            self.data_analytics.restart()
+        if self.inference_path:
+            free = queue.Queue()
+            for slot in range(3):
+                free.put(slot)
+            writer = VideoWriterThread(self.inference_path, self.video_info.fps, self.video_info.resolution_wh, free)
+            try:
+                renderer, batches = self._render_batches(frame_source, self.data_analytics, free)
+                for frames, slot in batches:
+                    writer.put(frames, slot)
+            finally:
+                writer.close()
+            self.timings["_render_encode"] = writer.seconds
+            for k, v in renderer.times.items():
+                self.timings[f"_render_{k}"] = v
+        else:  # data only: the positions need no frame
+            _, total = self._render_source(frame_source)
+            court = self.projected_court
+            court.H = None
+            for i in range(total):
+                players = keypoints = None
+                for t in self.trackers.values():
+                    if t.object() is Players:
+                        players = t.results[i]
+                    elif t.object() is Keypoints:
+                        keypoints = t.results[i]
+                H = court.update_homography(keypoints, self.is_fixed_keypoints)
+                if H is not None and players:
+                    court.project_players(players, H, self.data_analytics)
+                self.data_analytics.step(1)
+        if self.data_analytics is not None:  # q7: the reference trims even when it collects nothing
+            self.data_analytics.frames = self.data_analytics.frames[:-1]  # remove the extra frame
 
     # ---- fused single pass -------------------------------------------------------------------------------------
     def _ball_median(self, tracker: BallTracker, src, total: int, rank: int, dist_on: bool):
