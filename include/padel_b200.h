@@ -199,18 +199,19 @@ typedef struct pb_yolo_level {
 /* cand: float (B, cap, 6+nk) rows = x1,y1,x2,y2,conf,cls,kpts(raw decoded, network px); cand_count: int (B) (may
  * exceed cap: rows beyond cap are dropped, the caller checks).  Candidates are the anchors whose best class score is
  * > conf and, when `classes` (HOST array of n_classes ids, the `classes=` list of predict()) is not NULL, whose best
- * class is in it.                                                                                                */
+ * class is in it.  The best class is the first whose sigmoid score is the largest (ultralytics' cls.max(1)).     */
 int pb_yolo_decode(const pb_yolo_level* levels, int nlevels, int B, int fC, int nc, int nk, int kdim, int cls_off,
                    int kpt_off, float conf, const int* classes, int n_classes, float* cand, int* cand_anchor,
                    int* cand_count, int cap, void* stream);
-/* Per-image: sort by (conf desc, anchor asc), greedy NMS with IoU > iou suppression on class-offset boxes
- * (offset 7680*cls), keep first max_det. out: float (B, max_det, 6+nk); out_count int (B).
+/* Per-image: sort by (conf desc, anchor asc), greedy NMS on class-offset boxes (offset 7680*cls), keep first max_det,
+ * as torchvision.ops.nms: the float IoU in torchvision's op order, suppressed when (double)IoU > iou.
+ * out: float (B, max_det, 6+nk); out_count int (B).
  * cap <= 4096: everything in shared memory.  Larger capacities (ultralytics keeps up to max_nms = 30000 candidates,
  * cap <= 32768 here) need `scratch` = device buffer of pb_yolo_nms_scratch_bytes(B, cap) bytes, used only by images
  * that actually hold more than 4096 candidates.                                                                  */
 size_t pb_yolo_nms_scratch_bytes(int B, int cap);
 int pb_yolo_nms(const float* cand, const int* cand_anchor, const int* cand_count, int B, int cap, int rowlen,
-                float iou, int max_det, float* out, int* out_count, void* scratch, void* stream);
+                double iou, int max_det, float* out, int* out_count, void* scratch, void* stream);
 
 /* ---- ResNet50 court-keypoint regressor: the non-3x3/1x1 pieces (keypoints_tracker.py:158-167,276-312;
  *      keypoints_tracker/iterable.py:10-41).  The bottleneck stacks are pb_conv2d programs (res_before_act = 1). ---- */

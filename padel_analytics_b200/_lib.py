@@ -90,7 +90,7 @@ SIGNATURES = {
     "pb_yolo_decode": (_i, [C.POINTER(YoloLevel), _i, _i, _i, _i, _i, _i, _i, _i, _f, C.POINTER(C.c_int), _i, _p, _p, _p,
                              _i, _p]),
     "pb_yolo_nms_scratch_bytes": (C.c_size_t, [_i, _i]),
-    "pb_yolo_nms": (_i, [_p, _p, _p, _i, _i, _i, _f, _i, _p, _p, _p, _p]),
+    "pb_yolo_nms": (_i, [_p, _p, _p, _i, _i, _i, C.c_double, _i, _p, _p, _p, _p]),
     "pb_u8_normalize_f16": (_i, [_p, C.c_longlong, C.POINTER(C.c_float), C.POINTER(C.c_float), _p, _p]),
     "pb_resnet_stem7x7": (_i, [_p, _i, _i, _i, _p, _p, _p, _p]),
     "pb_maxpool3x3s2": (_i, [_p, _i, _i, _i, _i, _p, _p]),
