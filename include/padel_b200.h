@@ -190,6 +190,11 @@ int pb_u8_to_f16_nhwc16(const uint8_t* src, int B, int H, int W, void* dst, int 
  * x half NHWC (B,H,W,32): channels [med(3), f[first+b+0](3) ... f[first+b+7](3), 0 x5].                          */
 int pb_tracknet_pack_windows(const void* frames, int ring, int first_slot, const void* median, int B, int H, int W,
                              void* x, void* stream);
+/* Window assembly for a batch whose windows come from several clips: row b gathers the ring slots
+ * (row_slot[b] + f) % ring, f = 0..7, and the background medians[row_median[b]] (medians: (K,H,W,4) like median).
+ * row_slot, row_median: int (B) on the device.  Byte-identical to pb_tracknet_pack_windows on each row.           */
+int pb_tracknet_pack_windows_rows(const void* frames, int ring, const int* row_slot, const void* medians,
+                                  const int* row_median, int B, int H, int W, void* x, void* stream);
 
 /* ---- YOLOv8 head decode + NMS (ultralytics Detect/Pose decode, ops.non_max_suppression; SURVEY App. A.3-A.4) --- */
 typedef struct pb_yolo_level {
@@ -266,6 +271,14 @@ int pb_median_u8(const uint8_t* frames, int T, long long frame_bytes, uint8_t* o
  * mask: u8 (nframes,H,W) (0/1). ens (optional, may be NULL): float (nframes,H,W).                               */
 int pb_tracknet_ensemble(const float* pred, int S, int first_window, int total_windows, int frame0, int nframes,
                          int H, int W, float thr, uint8_t* mask, float* ens, void* stream);
+/* The same ensemble for frames of several clips in one launch.  pred row r holds global window first_window + r
+ * (windows of consecutive clips are consecutive).  desc: int (nframes,3) on the device, per output frame
+ * (global window index of its clip's first window, the clip's window count = clip frames - 7, the frame's index in
+ * the clip).  Each frame uses only its clip's windows and that clip's head/tail rules: the output equals
+ * pb_tracknet_ensemble run on each clip alone, bit for bit.  The caller guarantees that every window a frame needs
+ * is in pred.                                                                                                     */
+int pb_tracknet_ensemble_rows(const float* pred, int first_window, const int* desc, int nframes, int H, int W,
+                              float thr, uint8_t* mask, float* ens, void* stream);
 /* 8-connected components of each mask; picks the component with max bbox area (ties: the one whose first pixel in
  * raster order comes last, = cv2.findContours order + predict_location's strict '>' scan).
  * bbox: int (nframes,4) = x,y,w,h (0,0,0,0 if empty). scratch: int32 (nframes, 5, H*W).                          */

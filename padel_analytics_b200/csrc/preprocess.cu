@@ -307,6 +307,47 @@ __global__ void tracknet_pack_kernel(const uint2* __restrict__ frames, int ring,
   }
 }
 
+// The same gather, but row b takes its first ring slot from row_slot[b] and its background from
+// medians[row_median[b]]: a batch of windows that spans several clips (each clip has its own median, and the ring
+// skips the 7 frames at the end of a clip that start no window).
+__global__ void tracknet_pack_rows_kernel(const uint2* __restrict__ frames, int ring, const int* __restrict__ row_slot,
+                                          const uint2* __restrict__ medians, const int* __restrict__ row_median, int B,
+                                          int HW, uint4* __restrict__ x) {
+  const long total = (long)B * HW;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int pix = (int)(i % HW);
+    const int b = (int)(i / HW);
+    const int first_slot = __ldg(row_slot + b);
+    unsigned short h[32];
+    {
+      const uint2 m = __ldg(medians + (size_t)__ldg(row_median + b) * HW + pix);
+      h[0] = (unsigned short)(m.x & 0xFFFF);
+      h[1] = (unsigned short)(m.x >> 16);
+      h[2] = (unsigned short)(m.y & 0xFFFF);
+    }
+#pragma unroll
+    for (int f = 0; f < 8; ++f) {
+      const int slot = (first_slot + f) % ring;
+      const uint2 p = __ldg(frames + (size_t)slot * HW + pix);
+      h[3 + 3 * f] = (unsigned short)(p.x & 0xFFFF);
+      h[4 + 3 * f] = (unsigned short)(p.x >> 16);
+      h[5 + 3 * f] = (unsigned short)(p.y & 0xFFFF);
+    }
+#pragma unroll
+    for (int j = 27; j < 32; ++j) h[j] = 0;
+    uint4* o = x + i * 4;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      uint4 v;
+      v.x = (uint32_t)h[8 * q + 0] | ((uint32_t)h[8 * q + 1] << 16);
+      v.y = (uint32_t)h[8 * q + 2] | ((uint32_t)h[8 * q + 3] << 16);
+      v.z = (uint32_t)h[8 * q + 4] | ((uint32_t)h[8 * q + 5] << 16);
+      v.w = (uint32_t)h[8 * q + 6] | ((uint32_t)h[8 * q + 7] << 16);
+      o[q] = v;
+    }
+  }
+}
+
 static int grid_for(long total, int threads) {
   long b = (total + threads - 1) / threads;
   const long cap = (long)num_sms() * 32;
@@ -397,6 +438,20 @@ int pb_tracknet_pack_windows(const void* frames, int ring, int first_slot, const
   tracknet_pack_kernel<<<grid_for(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const uint2*>(frames), ring, first_slot, reinterpret_cast<const uint2*>(median), B, H * W,
       reinterpret_cast<uint4*>(x));
+  PB_CUDA(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+int pb_tracknet_pack_windows_rows(const void* frames, int ring, const int* row_slot, const void* medians,
+                                  const int* row_median, int B, int H, int W, void* x, void* stream) {
+  PB_CHECK(frames && row_slot && medians && row_median && x, "tracknet_pack_rows: null pointer");
+  PB_CHECK(ring >= 8, "tracknet_pack_rows: ring must hold at least 8 frames");
+  if (B <= 0) return 0;
+  const long total = (long)B * H * W;
+  tracknet_pack_rows_kernel<<<grid_for(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<const uint2*>(frames), ring, row_slot, reinterpret_cast<const uint2*>(medians), row_median, B,
+      H * W, reinterpret_cast<uint4*>(x));
   PB_CUDA(cudaGetLastError());
   count_launch();
   return 0;

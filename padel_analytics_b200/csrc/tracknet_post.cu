@@ -42,6 +42,44 @@ __global__ void ensemble_kernel(const float* __restrict__ pred, int S, int first
   }
 }
 
+// The same ensemble for frames of several clips in one launch.  desc[f] = (global pred row of the frame's clip's first
+// window, that clip's window count, the frame's index in its clip); pred row r holds global window first_window + r.
+// Each frame reads only its own clip's windows and applies the head/tail rules of that clip, with the arithmetic of
+// ensemble_kernel term for term.
+__global__ void ensemble_rows_kernel(const float* __restrict__ pred, int first_window, const int* __restrict__ desc,
+                                     int nframes, int HW, float thr, uint8_t* __restrict__ mask,
+                                     float* __restrict__ ens) {
+  const long total = (long)nframes * HW;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int pix = (int)(i % HW);
+    const int* d = desc + (i / HW) * 3;
+    const int base = __ldg(d) - first_window;  // pred row of the clip's window 0
+    const int total_windows = __ldg(d + 1);
+    const int n = __ldg(d + 2);  // frame index within the clip
+    float acc = 0.f;
+    float result;
+    if (n < total_windows && n >= 7) {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const float wk = (float)(k < 4 ? k + 1 : 8 - k) / 20.0f;
+        const int s = base + n - 7 + k;
+        acc = __fadd_rn(acc, __fmul_rn(pred[((size_t)s * 8 + (7 - k)) * HW + pix], wk));
+      }
+      result = acc;
+    } else {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const int w = n - 7 + k;
+        if (w >= 0 && w < total_windows) acc += pred[((size_t)(base + w) * 8 + (7 - k)) * HW + pix];
+      }
+      const float div = (n < total_windows) ? (float)(n + 1) : (float)(8 - (n - (total_windows - 1)));
+      result = acc / div;
+    }
+    mask[i] = result > thr ? 1 : 0;
+    if (ens) ens[i] = result;
+  }
+}
+
 __device__ __forceinline__ int uf_find(const int* parent, int i) {
   int p = __ldcg(parent + i);
   while (p != i) {
@@ -181,6 +219,21 @@ int pb_tracknet_ensemble(const float* pred, int S, int first_window, int total_w
   if (blocks > (long)num_sms() * 32) blocks = (long)num_sms() * 32;
   ensemble_kernel<<<(int)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       pred, S, first_window, total_windows, frame0, nframes, H * W, thr, mask, ens);
+  PB_CUDA(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+int pb_tracknet_ensemble_rows(const float* pred, int first_window, const int* desc, int nframes, int H, int W,
+                              float thr, uint8_t* mask, float* ens, void* stream) {
+  PB_CHECK(pred && desc && mask, "ensemble_rows: null pointer");
+  PB_CHECK((reinterpret_cast<uintptr_t>(desc) & 3) == 0, "ensemble_rows: desc must be 4-byte aligned");
+  if (nframes <= 0) return 0;
+  const long total = (long)nframes * H * W;
+  long blocks = (total + 255) / 256;
+  if (blocks > (long)num_sms() * 32) blocks = (long)num_sms() * 32;
+  ensemble_rows_kernel<<<(int)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      pred, first_window, desc, nframes, H * W, thr, mask, ens);
   PB_CUDA(cudaGetLastError());
   count_launch();
   return 0;

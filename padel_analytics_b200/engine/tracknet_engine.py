@@ -174,16 +174,8 @@ class BallPipeline:
     (ball_tracker.py:373-523) including its head/tail ensemble rules (SURVEY App. C)."""
 
     def __init__(self, engine: TrackNetEngine, frame_hw: tuple[int, int], median_rgb: np.ndarray | torch.Tensor):
-        self.eng = engine
-        self.dev = engine.device
-        self.Hs, self.Ws = frame_hw
-        B = engine.B
-        self.B = B
-        H, W = engine.H, engine.W
-        bh, kh, self.ksh = resample.pil_bicubic_tables(self.Ws, W)
-        bv, kv, self.ksv = resample.pil_bicubic_tables(self.Hs, H)
-        up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(self.dev)
-        self.bh, self.kh, self.bv, self.kv = up(bh), up(kh), up(bv), up(kv)
+        self._init_resize(engine, frame_hw)
+        B, H, W = self.B, engine.H, engine.W
         self.ring = B + 8
         # resized RGB frames as normalised fp16 4-channel pixels (what the window-packing kernel gathers from)
         self.small = torch.zeros((self.ring, H, W, 4), dtype=torch.float16, device=self.dev)
@@ -200,6 +192,17 @@ class BallPipeline:
         self._median_src = None
         self.set_median(median_rgb)
         self.reset()
+
+    def _init_resize(self, engine: TrackNetEngine, frame_hw):
+        """Engine, frame size and the Pillow bicubic tables (frame size -> network size) on the device."""
+        self.eng = engine
+        self.dev = engine.device
+        self.Hs, self.Ws = frame_hw
+        self.B = engine.B
+        bh, kh, self.ksh = resample.pil_bicubic_tables(self.Ws, engine.W)
+        bv, kv, self.ksv = resample.pil_bicubic_tables(self.Hs, engine.H)
+        up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(self.dev)
+        self.bh, self.kh, self.bv, self.kv = up(bh), up(kh), up(bv), up(kv)
 
     def set_median(self, median_rgb):
         """(Re)apply the background: full-res RGB -> uint8 -> PIL resize (iterable.py:76-81), on device with the same
@@ -297,6 +300,108 @@ class BallPipeline:
             if state["result"] is None:
                 done.synchronize()
                 state["result"] = (w0, host[:nframes].numpy().copy())
+                self._pending[slot] = None
+            return state["result"]
+
+        self._pending[slot] = finish
+        return finish
+
+
+class ClipBallPipeline(BallPipeline):
+    """BallPipeline over a list of clips in one stream: a device batch may hold the windows of several clips.  The
+    host plan (`clip_plan.plan_clip_batches`) says where each frame goes in the ring, when each clip's background is
+    loaded into the median pool and which windows every batch runs; the device gathers each row from its own ring slot
+    and median (`pb_tracknet_pack_windows_rows`) and ensembles each emitted frame over its own clip's windows only
+    (`pb_tracknet_ensemble_rows`).  Per clip the boxes are bit-identical to BallPipeline run on that clip alone."""
+
+    def __init__(self, engine: TrackNetEngine, frame_hw: tuple[int, int], ring: int | None = None,
+                 pool: int | None = None):
+        from .clip_plan import default_pool, default_ring
+
+        self._init_resize(engine, frame_hw)
+        B, H, W = self.B, engine.H, engine.W
+        self.ring = default_ring(B) if ring is None else ring
+        self.pool = default_pool(self.ring) if pool is None else pool
+        self.max_frames = 8 * B  # a window emits its own frame, plus the 7 tail frames when it ends its clip
+        self.small = torch.zeros((self.ring, H, W, 4), dtype=torch.float16, device=self.dev)
+        self.medians = torch.zeros((self.pool, H, W, 4), dtype=torch.float16, device=self.dev)
+        self.tmp = torch.zeros((B + 7, self.Hs, W, 3), dtype=torch.uint8, device=self.dev)
+        self.mask = torch.zeros((self.max_frames, H, W), dtype=torch.uint8, device=self.dev)
+        self.scratch = torch.zeros((B + 7, 5, H * W), dtype=torch.int32, device=self.dev)  # boxes run B+7 at a time
+        self.bbox = torch.zeros((self.max_frames, 4), dtype=torch.int32, device=self.dev)
+        self._host_ring = [torch.zeros((self.max_frames, 4), dtype=torch.int32).pin_memory() for _ in range(3)]
+        self._pending = [None] * 3
+        self._turn = 0
+        self.plan = None
+
+    def begin(self, plan) -> None:
+        """Upload every batch's row and frame tables of `plan` (a ClipPlan with this ring and pool) at once."""
+        if plan.ring != self.ring or plan.pool != self.pool or plan.batch > self.B or plan.chunk > self.B:
+            raise L.PbError("ClipBallPipeline: the plan was made for another ring, pool or batch size")
+        rows, desc, self._tables = [], [], []
+        for ops in plan.steps:
+            for op in ops:
+                if op[0] == "run":
+                    b = op[1]
+                    self._tables.append((len(rows), len(desc)))
+                    rows += list(zip(b.row_slot, b.row_median))
+                    desc += b.desc
+        rows_t = torch.tensor(rows or [(0, 0)], dtype=torch.int32).t().contiguous()
+        self._rows = rows_t.to(self.dev)  # (2, windows): ring slot, median slot
+        self._desc = torch.tensor(desc or [(0, 0, 0)], dtype=torch.int32).to(self.dev)
+        self._next_run = 0
+        self.plan = plan
+        self.eng.pred.zero_()
+
+    def load_median(self, slot: int, median_rgb: torch.Tensor) -> None:
+        """(Hs,Ws,3) uint8 RGB background (device) -> resized into pool slot `slot`, as BallPipeline.set_median does."""
+        med = median_rgb.to(self.dev, torch.uint8).contiguous().view(1, self.Hs, self.Ws, 3)
+        self._resize(med, 1, self.medians[slot:slot + 1], swap_rb=0)
+
+    def push_at(self, frames_bgr: torch.Tensor, slot: int) -> None:
+        """Resize (n,Hs,Ws,3) uint8 BGR device frames into ring slots slot..slot+n-1."""
+        n = frames_bgr.shape[0]
+        if n and (slot + n > self.ring or n > self.B + 7):
+            raise L.PbError("ClipBallPipeline: push outside the ring")
+        if n:
+            self._resize(frames_bgr.contiguous(), n, self.small[slot:slot + n], swap_rb=1)
+
+    def run_batch_async(self, batch):
+        """Enqueue one planned batch; returns a callable that waits and yields (frames [(clip, frame)], host int32
+        (nframes, 4) boxes)."""
+        eng = self.eng
+        nb, nframes = len(batch.windows), len(batch.frames)
+        r0, d0 = self._tables[self._next_run]
+        self._next_run += 1
+        rows = self._rows[:, r0:r0 + nb]
+        L.check(L.lib().pb_tracknet_pack_windows_rows(self.small.data_ptr(), self.ring, rows[0].data_ptr(),
+                                                      self.medians.data_ptr(), rows[1].data_ptr(), nb, eng.H, eng.W,
+                                                      eng.x.data_ptr(), L.stream_ptr()))
+        eng.run_packed()
+        L.check(L.lib().pb_tracknet_ensemble_rows(eng.pred.data_ptr(), batch.first_window - 7,
+                                                  self._desc[d0:d0 + nframes].data_ptr(), nframes, eng.H, eng.W, 0.5,
+                                                  self.mask.data_ptr(), None, L.stream_ptr()))
+        step = self.scratch.shape[0]
+        for f in range(0, nframes, step):  # the scratch holds B+7 frames: several launches for the short-clip case
+            n = min(step, nframes - f)
+            L.check(L.lib().pb_ccl_bbox(self.mask[f:].data_ptr(), n, eng.H, eng.W, self.scratch.data_ptr(),
+                                        self.bbox[f:].data_ptr(), L.stream_ptr()))
+        slot = self._turn
+        self._turn = (slot + 1) % len(self._host_ring)
+        if self._pending[slot] is not None:
+            self._pending[slot]()
+        host = self._host_ring[slot]
+        host[:nframes].copy_(self.bbox[:nframes], non_blocking=True)
+        carry = eng.pred[nb:nb + 7].clone()  # the last 7 windows, for the next batch (which may start another clip)
+        eng.pred[:7].copy_(carry)
+        done = torch.cuda.Event()
+        done.record()
+        state = {"result": None}
+
+        def finish():
+            if state["result"] is None:
+                done.synchronize()
+                state["result"] = (batch.frames, host[:nframes].numpy().copy())
                 self._pending[slot] = None
             return state["result"]
 

@@ -21,7 +21,7 @@ import numpy as np
 import torch
 
 from ..engine.inpaint_engine import InpaintNetEngine
-from ..engine.tracknet_engine import BallPipeline, TrackNetEngine, bbox_to_xyv
+from ..engine.tracknet_engine import BallPipeline, ClipBallPipeline, TrackNetEngine, bbox_to_xyv
 from .tracker import NoPredictSample, Object, Tracker
 
 
@@ -62,6 +62,12 @@ def median_background(frames_bgr, device="cuda") -> np.ndarray:
     arrays, or one (T,H,W,3) uint8 tensor, host or device) are stacked in HBM and `pb_median_u8` selects the per-byte
     median (even counts: mean of the two middle values, truncated like the reference's float64 -> uint8 cast),
     writing RGB order.  Returns the (H,W,3) uint8 RGB median on the host."""
+    return median_background_device(frames_bgr, device).cpu().numpy()
+
+
+def median_background_device(frames_bgr, device="cuda") -> torch.Tensor:
+    """`median_background` without the download: the (H,W,3) uint8 RGB median stays on the device, computed on the
+    current stream."""
     from .. import _lib as L
 
     if isinstance(frames_bgr, torch.Tensor):
@@ -78,7 +84,7 @@ def median_background(frames_bgr, device="cuda") -> np.ndarray:
     T, H, W, _ = stack.shape
     out = torch.empty((H, W, 3), dtype=torch.uint8, device=stack.device)
     L.check(L.lib().pb_median_u8(stack.data_ptr(), T, H * W * 3, out.data_ptr(), 1, L.stream_ptr()))
-    return out.cpu().numpy()
+    return out
 
 
 class BallTracker(Tracker):
@@ -114,6 +120,7 @@ class BallTracker(Tracker):
         self.median_max_sample_num = median_max_sample_num
         self.median = median
         self._pipe = None
+        self._clip_pipe = None
 
     def video_info_post_init(self, video_info) -> "BallTracker":
         self.video_info = video_info
@@ -214,9 +221,54 @@ class BallTracker(Tracker):
                             scaler=(self.video_info.width / self.WIDTH, self.video_info.height / self.HEIGHT))
         return pipe
 
+    def clips_begin(self, frame_hw, plan, median_of):
+        """Streaming over a list of clips (`TrackingRunner.run_clips`): `plan` is the ClipPlan of the stream
+        (`clip_plan.plan_clip_batches` with this tracker's ring and pool, see `clip_pipeline`); `median_of(clip)`
+        returns (device (H,W,3) uint8 RGB background, CUDA event after which it is ready, or None).  Each
+        `stream_push_async` then takes the next upload chunk and its finish yields [(clip, frame, (x, y, vis))]."""
+        pipe = self.clip_pipeline(frame_hw)
+        pipe.begin(plan)
+        self._stream = dict(clips=plan, step=0, median_of=median_of,
+                            scaler=(frame_hw[1] / self.WIDTH, frame_hw[0] / self.HEIGHT))
+        return pipe
+
+    def clip_pipeline(self, frame_hw) -> ClipBallPipeline:
+        if self._clip_pipe is None or (self._clip_pipe.Hs, self._clip_pipe.Ws) != tuple(frame_hw):
+            self._clip_pipe = ClipBallPipeline(self.tracknet, tuple(frame_hw))
+        return self._clip_pipe
+
+    def _clips_push_async(self, frames: torch.Tensor):
+        pipe, s = self._clip_pipe, self._stream
+        ops = s["clips"].steps[s["step"]]
+        s["step"] += 1
+        fins = []
+        for op in ops:
+            if op[0] == "median":
+                med, ready = s["median_of"](op[1])
+                if ready is not None:
+                    torch.cuda.current_stream().wait_event(ready)
+                pipe.load_median(op[2], med)
+            elif op[0] == "push":
+                _, off, n, slot = op
+                pipe.push_at(frames[off:off + n], slot)
+            else:
+                fins.append(pipe.run_batch_async(op[1]))
+
+        def finish():
+            out = []
+            for fin in fins:
+                frames_cf, bbox = fin()
+                xs, ys, vs = bbox_to_xyv(bbox, s["scaler"])
+                out += [(c, f, (xs[i], ys[i], vs[i])) for i, (c, f) in enumerate(frames_cf)]
+            return out
+
+        return finish
+
     def stream_push_async(self, frames: torch.Tensor):
         """frames: uint8 (n,H,W,3) BGR tensor (device or pinned host), n <= batch_size.  Enqueues resize + every
         window that became computable; returns a callable that waits and yields {frame: (x, y, vis)}."""
+        if "clips" in self._stream:
+            return self._clips_push_async(frames)
         pipe, s = self._pipe, self._stream
         pipe.push_frames(frames)
         fins = []

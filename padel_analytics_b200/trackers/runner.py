@@ -75,7 +75,10 @@ class FusedPass:
                         for _ in range(2)]
         self.ready = [torch.cuda.Event(), torch.cuda.Event()]
         self.consumed = [None, None]  # per staging slot: event after the device work that read it
-        for t in trackers.values():
+        self._begin_ball(total_frames, first_frame, emit_range, median)
+
+    def _begin_ball(self, total_frames, first_frame, emit_range, median) -> None:
+        for t in self.trackers.values():
             if isinstance(t, BallTracker):
                 t.stream_begin(self.hw, total_frames, first_frame, emit_range, median=median)
 
@@ -177,6 +180,77 @@ class FusedPass:
             nrec = start(nxt, i + 1) if nxt is not None else None
             yield self._finish(rec)
             rec, i = nrec, i + 1
+
+
+class ClipPass(FusedPass):
+    """FusedPass over a list of clips played back to back: upload chunk i holds frames [i*B, (i+1)*B) of the
+    concatenated clips, so device batches stay full across clip boundaries.  The ball tracker runs its windows by the
+    clip plan (`clip_plan.plan_clip_batches`: a window never spans two clips, each clip has its own background), and
+    the order-dependent host stages restart per clip: at a clip's first frame each YOLO tracker gets the clip's
+    video_info (PlayerTracker: a fresh ByteTrack at the clip's fps).  Per batch, `run` yields {tracker name:
+    [(clip, results of that clip's frames in the batch)]} for the YOLO trackers and [(clip, frame, (x, y, vis))] for
+    the ball tracker, whose frames may come late (its partial batches wait for more windows)."""
+
+    def __init__(self, trackers: dict[str, Tracker], frame_hw: tuple[int, int], batch_size: int, lengths: list[int],
+                 clip_infos: list, median_of: Callable, streams: Optional[int] = None):
+        self.lengths = list(lengths)
+        self.clip_infos = clip_infos
+        self.median_of = median_of
+        self._starts = np.cumsum([0] + self.lengths)
+        self._pos = 0
+        super().__init__(trackers, frame_hw, batch_size, total_frames=int(self._starts[-1]), streams=streams)
+
+    def _begin_ball(self, total_frames, first_frame, emit_range, median) -> None:
+        from ..engine.clip_plan import plan_clip_batches
+
+        for t in self.trackers.values():
+            if isinstance(t, BallTracker):
+                pipe = t.clip_pipeline(self.hw)
+                plan = plan_clip_batches(self.lengths, t.batch_size, chunk=self.B, ring=pipe.ring, pool=pipe.pool)
+                t.clips_begin(self.hw, plan, self.median_of)
+
+    def _upload(self, pieces, slot: int) -> torch.Tensor:
+        """pieces: uint8 (n,H,W,3) tensors (pinned host or device) that make up one chunk, in order."""
+        if isinstance(pieces, torch.Tensor):
+            pieces = [pieces]
+        if len(pieces) == 1 and pieces[0].device.type == "cuda":
+            return pieces[0]
+        n = sum(p.shape[0] for p in pieces)
+        main = torch.cuda.current_stream()
+        with torch.cuda.stream(self.copy_stream):
+            if self.consumed[slot] is not None:
+                self.copy_stream.wait_event(self.consumed[slot])
+            if any(p.device.type == "cuda" for p in pieces):
+                self.copy_stream.wait_stream(main)
+            at = 0
+            for p in pieces:
+                self.staging[slot][at:at + p.shape[0]].copy_(p, non_blocking=True)
+                at += p.shape[0]
+            self.ready[slot].record(self.copy_stream)
+        return self.staging[slot][:n]
+
+    def _finish(self, launched) -> dict:
+        pending, nfr = launched
+        base, segs, lo = self._pos, [], self._pos
+        while lo < base + nfr:  # (clip, first, end) in the chunk, and the clip frame at `first`
+            c = int(np.searchsorted(self._starts, lo, side="right")) - 1
+            e = min(base + nfr, int(self._starts[c + 1]))
+            segs.append((c, lo - base, e - base, lo - int(self._starts[c])))
+            lo = e
+        self._pos = base + nfr
+        out = {}
+        for name, t, fin in pending:
+            if isinstance(t, BallTracker):
+                out[name] = fin()
+                continue
+            res, parts = fin(), []
+            for c, a, b, f0 in segs:
+                if f0 == 0:
+                    t.video_info_post_init(self.clip_infos[c])
+                piece = res[a:b]
+                parts.append((c, t.postprocess(piece) if isinstance(t, PlayerTracker) else t.postprocess(piece, self.hw)))
+            out[name] = parts
+        return out
 
 
 class TrackingRunner:
@@ -526,6 +600,214 @@ class TrackingRunner:
                 tracker.results.predictions = tracker.postprocess(results, hw)
         else:
             tracker.results.predictions = [o for p in parts for o in p]
+
+    # ---- a list of clips in one pass ----------------------------------------------------------------------------
+    def run_clips(self, clips: list, save_dir: Optional[str] = None, streams: Optional[int] = None) -> list[dict]:
+        """Track a list of clips in one pass and return, per clip, {tracker name: list[Object]}: the results a fresh
+        `TrackingRunner(trackers, video_info=<the clip's>).run()` gives on that clip alone.
+
+        clips: video paths, or (frame_source, total_frames) pairs where frame_source(lo, hi) yields the clip's frames
+        lo..hi-1 as HWC uint8 BGR frames or (n,H,W,3) uint8 batches (pinned host or device tensors); pairs take
+        their fps from this runner's video_info.  Every clip must have the frame size of the first one.
+
+        The clips are played back to back through one `ClipPass` (one upload per batch, one batch of look-ahead, the
+        stream modes of FusedPass), so device batches stay full across clip boundaries and the next clip decodes
+        while the device works.  Per clip: the ball background is the median of the clip's first
+        `median_max_sample_num` frames (unless the BallTracker has a fixed `median`), InpaintNet runs over the clip's
+        trajectory, and ByteTrack restarts at the clip's fps.  Trackers with a fixed keypoints detection repeat it.
+        With `save_dir`, each clip's predictions are written as `<save_dir>/<clip:04d>_<tracker>.json` in the format
+        of `save_predictions`.  The trackers' own `results` are left untouched."""
+        import gc
+
+        gc_was_on = gc.isenabled()
+        gc.disable()
+        try:
+            out = self._run_clips(clips, streams)
+        finally:
+            if gc_was_on:
+                gc.enable()
+        if save_dir is not None:
+            import json
+
+            os.makedirs(save_dir, exist_ok=True)
+            for c, res in enumerate(out):
+                for name, objs in res.items():
+                    with open(os.path.join(save_dir, f"{c:04d}_{name}.json"), "w") as f:
+                        json.dump([o.serialize() for o in objs], f)
+        return out
+
+    def _run_clips(self, clips: list, streams: Optional[int]) -> list[dict]:
+        import itertools
+
+        from .ball_tracker import median_background_device
+
+        srcs, lengths, fps, hw = [], [], [], None
+        for i, clip in enumerate(clips):
+            if isinstance(clip, (str, os.PathLike)):
+                vi = sv.VideoInfo.from_video_path(str(clip))
+                srcs.append((lambda p: lambda lo, hi: sv.get_video_frames_generator(p, start=lo, end=hi))(str(clip)))
+                lengths.append(int(vi.total_frames))
+                fps.append(vi.fps)
+                if hw is None:
+                    hw = (vi.height, vi.width)
+                elif (vi.height, vi.width) != hw:
+                    raise ValueError(f"clip {i} is {vi.width}x{vi.height}, clip 0 is {hw[1]}x{hw[0]}: "
+                                     "all clips of one call must have the same frame size")
+            else:
+                src, total = clip
+                if self.video_info is None:
+                    raise ValueError("clips given as (frame_source, total_frames) take their fps from the runner's "
+                                     "video_info, and this runner has none")
+                srcs.append(src)
+                lengths.append(int(total))
+                fps.append(self.video_info.fps)
+        if any(t < 0 for t in lengths):
+            raise ValueError("clip lengths must be >= 0")
+        fixed = {n: t for n, t in self.trackers.items() if getattr(t, "fixed_keypoints_detection", None) is not None}
+        model = {n: t for n, t in self.trackers.items() if n not in fixed and (
+            isinstance(t, (PlayerTracker, PlayerKeypointsTracker, BallTracker)) or
+            (isinstance(t, KeypointsTracker) and t.model is not None))}
+        other = set(self.trackers) - set(fixed) - set(model)
+        if other:
+            raise ValueError(f"run_clips: trackers {sorted(other)} have neither a model nor a fixed detection")
+        out = [{n: [t.fixed_keypoints_detection] * T for n, t in fixed.items()} for T in lengths]
+        if not model or not sum(lengths):
+            for res, T in zip(out, lengths):
+                res.update({n: [] for n in model})
+            return out
+        ball_name, ball = next(((n, t) for n, t in model.items() if isinstance(t, BallTracker)), (None, None))
+        B = min(t.batch_size for t in model.values())
+        side = torch.cuda.Stream()  # backgrounds of the clips ahead are computed beside the pass
+        meds: dict = {}
+        shape = {"hw": hw}
+
+        def frame_count(item) -> int:
+            return item.shape[0] if isinstance(item, torch.Tensor) and item.dim() == 4 else 1
+
+        def items_of(c):
+            """clip c's frames as (n,H,W,3) uint8 tensors, after queueing its background when it needs one"""
+            it = iter(srcs[c](0, lengths[c]))
+            head = []
+            if ball is not None and lengths[c] >= 8:
+                if ball.median is not None:
+                    if "fixed" not in meds:
+                        meds["fixed"] = (torch.as_tensor(ball.median).to(torch.uint8).cuda(), None)
+                    meds[c] = meds["fixed"]
+                else:  # iterable.py:58-73 per clip, as TrackingRunner._ball_median does for one video
+                    m, got = min(lengths[c], ball.median_max_sample_num), 0
+                    for item in it:
+                        head.append(item)
+                        got += frame_count(item)
+                        if got >= m:
+                            break
+                    with torch.cuda.stream(side):
+                        if head and isinstance(head[0], torch.Tensor) and head[0].dim() == 4:
+                            med = median_background_device(torch.cat([h.to("cuda") for h in head])[:m])
+                        else:
+                            med = median_background_device([np.asarray(h) for h in head[:m]])
+                        ready = torch.cuda.Event()
+                        ready.record(side)
+                    meds[c] = (med, ready)
+            seen = 0
+            for item in itertools.chain(head, it):
+                t = item if isinstance(item, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(item))
+                if t.dim() == 3:
+                    t = t.unsqueeze(0)
+                if shape["hw"] is None:
+                    shape["hw"] = tuple(t.shape[1:3])
+                if tuple(t.shape[1:3]) != shape["hw"]:
+                    raise ValueError(f"clip {c} has {tuple(t.shape[1:3])} frames, the first clip "
+                                     f"{shape['hw']}: all clips of one call must have the same frame size")
+                t = t[:lengths[c] - seen]
+                seen += t.shape[0]
+                if t.shape[0]:
+                    yield t
+                if seen == lengths[c]:
+                    break
+            if seen != lengths[c]:
+                raise ValueError(f"clip {c} yielded {seen} frames, {lengths[c]} announced")
+
+        pinned = []
+
+        def chunks():
+            """upload chunks of B frames of the concatenated clips, as lists of pieces: host frames are gathered in
+            pinned buffers (three, reused: a chunk's buffer is refilled only after its results were yielded), batch
+            tensors are passed as slices"""
+            pieces, n, k, run0 = [], 0, 0, None
+            for c in range(len(srcs)):
+                for t in items_of(c):
+                    while t.shape[0]:
+                        take = min(B - n, t.shape[0])
+                        part, t = t[:take], t[take:]
+                        if part.device.type == "cuda" or part.is_pinned():
+                            if run0 is not None:
+                                pieces.append(pinned[k % 3][run0:n])
+                                run0 = None
+                            pieces.append(part)
+                        else:
+                            if not pinned:
+                                pinned.extend(torch.empty((B,) + shape["hw"] + (3,), dtype=torch.uint8).pin_memory()
+                                              for _ in range(3))
+                            pinned[k % 3][n:n + take].copy_(part)
+                            run0 = n if run0 is None else run0
+                        n += take
+                        if n == B:
+                            if run0 is not None:
+                                pieces.append(pinned[k % 3][run0:n])
+                            yield pieces
+                            pieces, n, k, run0 = [], 0, k + 1, None
+            if n:
+                if run0 is not None:
+                    pieces.append(pinned[k % 3][run0:n])
+                yield pieces
+
+        saved = {n: {k: t.__dict__[k] for k in ("video_info", "byte_track") if k in t.__dict__}
+                 for n, t in model.items()}  # the per-clip stages below replace these; run() finds them as they were
+        for t in model.values():
+            t.to(t.DEVICE)
+        t0 = timeit.default_timer()
+        gen = chunks()
+        first = next(gen)
+        hw = shape["hw"]
+        infos = [sv.VideoInfo(width=hw[1], height=hw[0], fps=f, total_frames=T) for f, T in zip(fps, lengths)]
+        fp = ClipPass(model, hw, B, lengths, infos, lambda c: meds[c], streams=streams)
+        yolo = {n: [[] for _ in lengths] for n in model if n != ball_name}
+        xyv = [{} for _ in lengths]
+        left = [T if T >= 8 else 0 for T in lengths]
+        inpaint_stream = torch.cuda.Stream()
+
+        def finish_ball(c):
+            """InpaintNet over the clip's trajectory (on a stream of its own: the pass keeps running) -> Ball list"""
+            ball.video_info = infos[c]
+            with torch.cuda.stream(inpaint_stream):
+                v = ball.inpaint_xyv(xyv[c], lengths[c])
+            out[c][ball_name] = [Ball(frame=n, xy=(v[n][0], v[n][1]), visibility=v[n][2]) if n in v
+                                 else Ball(frame=n, xy=(0.0, 0.0), visibility=0) for n in range(lengths[c])]
+
+        for res in fp.run(itertools.chain([first], gen)):
+            for name, parts in res.items():
+                if name == ball_name:
+                    for c, f, v in parts:
+                        xyv[c][f] = v
+                        left[c] -= 1
+                        if left[c] == 0:
+                            finish_ball(c)
+                else:
+                    for c, objs in parts:
+                        yolo[name][c] += objs
+        torch.cuda.synchronize()
+        if ball is not None:
+            for c, T in enumerate(lengths):
+                if ball_name not in out[c]:  # clips of fewer than 8 frames have no window
+                    finish_ball(c)
+        for name, per_clip in yolo.items():
+            for c, objs in enumerate(per_clip):
+                out[c][name] = objs
+        for n, t in model.items():
+            t.__dict__.update(saved[n])
+            t.to("cpu")
+        self.timings["_clips_pass"] = timeit.default_timer() - t0
+        return [{n: res[n] for n in self.trackers} for res in out]
 
 
 # ---- fixed-capacity records for the gather (SURVEY §8e) ---------------------------------------------------------
