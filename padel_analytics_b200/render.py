@@ -18,6 +18,7 @@ import functools
 import queue
 import threading
 import timeit
+from dataclasses import dataclass
 from typing import Callable, Iterable, Optional
 
 import numpy as np
@@ -156,9 +157,10 @@ class DisplayListBuilder:
         return x0, y0, x1 - x0, y1 - y0, sprite, _colour_bgr(p["color"])
 
     def frame_records(self, frame_index: int, trackers: dict, data_analytics: Optional[DataAnalytics],
-                      is_fixed_keypoints: bool) -> list:
+                      is_fixed_keypoints: bool, results: Optional[dict] = None) -> list:
         """Records of one frame: [(x0, y0, w, h, sprite or None (BLEND), colour)].  Updates the court's homography
-        and records the players' positions in `data_analytics` as the reference's pass does."""
+        and records the players' positions in `data_analytics` as the reference's pass does.  `results` maps each
+        tracker's name to the per-frame predictions to draw (default: the tracker's own `results`)."""
         import cv2
 
         from .trackers.ball_tracker import Ball
@@ -169,8 +171,8 @@ class DisplayListBuilder:
                               "fontFace": cv2.FONT_HERSHEY_SIMPLEX, "fontScale": 1, "color": FRAME_TEXT_COLOUR,
                               "thickness": 1})]
         players = ball = keypoints = None
-        for t in trackers.values():
-            pred = t.results[frame_index]
+        for name, t in trackers.items():
+            pred = (t.results if results is None else results[name])[frame_index]
             calls += record_draw_calls(pred.draw, **t.draw_kwargs())
             obj = t.object()
             if obj is Players:
@@ -406,7 +408,8 @@ def frame_batches(frames: Iterable, batch_size: int) -> Iterable:
 
 class VideoWriterThread:
     """cv2.VideoWriter on a thread of its own, so that encoding overlaps the next batch.  Batches come in as
-    (frames, out_slot); the slot goes back to `free_slots` once its frames are written."""
+    (frames, out_slot); the slot goes back to `free_slots` (anything with `put(slot)`) once its frames are written.
+    After `finish()` the thread writes what is queued, releases the writer and sets `closed`."""
 
     def __init__(self, path: str, fps: float, resolution_wh: tuple[int, int], free_slots: queue.Queue):
         import cv2
@@ -418,6 +421,8 @@ class VideoWriterThread:
         self.work: queue.Queue = queue.Queue()
         self.error = None
         self.seconds = 0.0
+        self.closed = threading.Event()
+        self._finished = False
         self.thread = threading.Thread(target=self._loop, daemon=True)
         self.thread.start()
 
@@ -436,13 +441,131 @@ class VideoWriterThread:
                     self.error = e
             self.seconds += timeit.default_timer() - t0
             self.free.put(slot)
+        try:
+            self.writer.release()
+        except Exception as e:
+            self.error = self.error or e
+        self.closed.set()
 
     def put(self, frames, slot: int):
         self.work.put((frames, slot))
 
+    def finish(self):
+        """No more frames: the writer is released once the queued ones are written, without waiting here."""
+        if not self._finished:
+            self._finished = True
+            self.work.put(None)
+
     def close(self):
-        self.work.put(None)
+        self.finish()
         self.thread.join()
-        self.writer.release()
         if self.error is not None:
             raise self.error
+
+
+# ---- a list of clips through one render pass ---------------------------------------------------------------------
+MAX_OPEN_WRITERS = 4  # encoders of consecutive clips that may run at once
+
+
+@dataclass(frozen=True)
+class ClipPart:
+    """Rows [lo, hi) of a batch: frames first.. of `clip`, for that clip's writer.  `open`: the writer is opened here
+    (the clip's first frame), after the writer of clip `wait` has closed when `wait` is not None.  `close`: the
+    clip's last frame, the writer is finished after this part."""
+    clip: int
+    lo: int
+    hi: int
+    first: int
+    open: bool
+    wait: Optional[int]
+    close: bool
+
+
+@dataclass(frozen=True)
+class ClipRenderBatch:
+    """One render batch of the concatenated clips: (clip, frame in clip) per row, and one part per clip with frames
+    in it.  The batch's out slot is free again once every part has been written."""
+    rows: list
+    parts: list
+
+
+def plan_clip_render(lengths: list[int], batch_size: int, max_open: int = MAX_OPEN_WRITERS) -> list[ClipRenderBatch]:
+    """Batches of `batch_size` frames over the clips played back to back (the last one partial).  Clips of 0 frames
+    have no rows and no writer.  A writer opens only after the one opened `max_open` opens before it has closed, so at
+    most `max_open` are open at once."""
+    if batch_size < 1 or max_open < 1:
+        raise ValueError("batch_size and max_open must be >= 1")
+    batches, rows, parts, opened = [], [], [], []
+    for c, T in enumerate(lengths):
+        f = 0
+        while f < T:
+            take = min(T - f, batch_size - len(rows))
+            wait = None
+            if f == 0:
+                wait = opened[-max_open] if len(opened) >= max_open else None
+                opened.append(c)
+            parts.append(ClipPart(c, len(rows), len(rows) + take, f, f == 0, wait, f + take == T))
+            rows += [(c, f + j) for j in range(take)]
+            f += take
+            if len(rows) == batch_size:
+                batches.append(ClipRenderBatch(rows, parts))
+                rows, parts = [], []
+    if rows:
+        batches.append(ClipRenderBatch(rows, parts))
+    return batches
+
+
+class _SlotRelease:
+    """Puts an out slot back on `free` after the last of the parts its batch was split into is written."""
+
+    def __init__(self, free: queue.Queue):
+        self.free, self.left, self.lock = free, {}, threading.Lock()
+
+    def expect(self, slot: int, parts: int):
+        with self.lock:
+            self.left[slot] = parts
+
+    def put(self, slot: int):
+        with self.lock:
+            self.left[slot] -= 1
+            done = self.left[slot] == 0
+        if done:
+            self.free.put(slot)
+
+
+def write_clip_batches(plan: list[ClipRenderBatch], batches: Iterable, open_writer: Callable,
+                       free_slots: queue.Queue) -> float:
+    """Writes the rendered batches ((frames, out slot) pairs, in `plan` order) to one writer per clip.
+    open_writer(clip, release) -> a started `VideoWriterThread` that hands slots to `release`.  Each clip's writer is
+    finished after its last part, so it drains while later clips render.  Every writer is closed before this returns;
+    the first error is raised after that.  Returns the writers' encode seconds."""
+    release = _SlotRelease(free_slots)
+    writers: dict = {}
+    error = None
+    n = 0
+    try:
+        for frames, slot in batches:
+            b = plan[n]
+            if len(frames) != len(b.rows):
+                raise ValueError(f"render batch {n} has {len(frames)} frames, the plan {len(b.rows)}")
+            release.expect(slot, len(b.parts))
+            for p in b.parts:
+                if p.open:
+                    if p.wait is not None:
+                        writers[p.wait].closed.wait()
+                    writers[p.clip] = open_writer(p.clip, release)
+                writers[p.clip].put(frames[p.lo:p.hi], slot)
+                if p.close:
+                    writers[p.clip].finish()
+            n += 1
+        if n != len(plan):
+            raise ValueError(f"{n} render batches, the plan has {len(plan)}")
+    finally:
+        for w in writers.values():
+            try:
+                w.close()
+            except Exception as e:
+                error = error or e
+    if error is not None:
+        raise error
+    return sum(w.seconds for w in writers.values())

@@ -4,7 +4,8 @@ detections are gathered once per tracker and the sequential host stages (ByteTra
 
 After the trackers, `run()` renders the annotated video to `inference_path` and collects the players' court positions
 into `data_analytics` (runner.py:91-173) when either is asked for; the overlays are composited on the device
-(render.py, `pb_render_overlay`) and encoding runs on a thread of its own.
+(render.py, `pb_render_overlay`) and encoding runs on a thread of its own.  `run_clips()` does the same per clip for a
+list of clips, in one render pass over the clips played back to back.
 
 Documented deviations from reference quirks (SURVEY App. E):
   q7  with collect_data=False the reference's drawing pass ends by trimming `self.data_analytics.frames`, which is
@@ -278,6 +279,7 @@ class TrackingRunner:
         self.projected_court = ProjectedCourt(video_info) if video_info is not None else None
         self.data_analytics = DataAnalytics() if collect_data else None
         self.render_batch_size = 32
+        self.clips_data_analytics: list[DataAnalytics] = []  # per clip, filled by run_clips(collect_data=True)
         self._source = None  # (frame_source, total_frames) of the last run(), for the drawing pass
         self.timings: dict[str, float] = {}
 
@@ -437,21 +439,27 @@ class TrackingRunner:
                 self.timings[f"_render_{k}"] = v
         else:  # data only: the positions need no frame
             _, total = self._render_source(frame_source)
-            court = self.projected_court
-            court.H = None
-            for i in range(total):
-                players = keypoints = None
-                for t in self.trackers.values():
-                    if t.object() is Players:
-                        players = t.results[i]
-                    elif t.object() is Keypoints:
-                        keypoints = t.results[i]
-                H = court.update_homography(keypoints, self.is_fixed_keypoints)
-                if H is not None and players:
-                    court.project_players(players, H, self.data_analytics)
-                self.data_analytics.step(1)
+            self._collect_positions({n: t.results for n, t in self.trackers.items()}, total, self.projected_court,
+                                    self.data_analytics)
         if self.data_analytics is not None:  # q7: the reference trims even when it collects nothing
             self.data_analytics.frames = self.data_analytics.frames[:-1]  # remove the extra frame
+
+    def _collect_positions(self, results: dict, total: int, court: ProjectedCourt,
+                           data_analytics: DataAnalytics) -> None:
+        """The players' court positions of frames 0..total-1 into `data_analytics`, without drawing.  results:
+        {tracker name: per-frame predictions}."""
+        court.H = None
+        for i in range(total):
+            players = keypoints = None
+            for name, t in self.trackers.items():
+                if t.object() is Players:
+                    players = results[name][i]
+                elif t.object() is Keypoints:
+                    keypoints = results[name][i]
+            H = court.update_homography(keypoints, self.is_fixed_keypoints)
+            if H is not None and players:
+                court.project_players(players, H, data_analytics)
+            data_analytics.step(1)
 
     # ---- fused single pass -------------------------------------------------------------------------------------
     def _ball_median(self, tracker: BallTracker, src, total: int, rank: int, dist_on: bool):
@@ -602,7 +610,8 @@ class TrackingRunner:
             tracker.results.predictions = [o for p in parts for o in p]
 
     # ---- a list of clips in one pass ----------------------------------------------------------------------------
-    def run_clips(self, clips: list, save_dir: Optional[str] = None, streams: Optional[int] = None) -> list[dict]:
+    def run_clips(self, clips: list, save_dir: Optional[str] = None, streams: Optional[int] = None,
+                  inference_dir: Optional[str] = None, collect_data: bool = False) -> list[dict]:
         """Track a list of clips in one pass and return, per clip, {tracker name: list[Object]}: the results a fresh
         `TrackingRunner(trackers, video_info=<the clip's>).run()` gives on that clip alone.
 
@@ -616,16 +625,39 @@ class TrackingRunner:
         `median_max_sample_num` frames (unless the BallTracker has a fixed `median`), InpaintNet runs over the clip's
         trajectory, and ByteTrack restarts at the clip's fps.  Trackers with a fixed keypoints detection repeat it.
         With `save_dir`, each clip's predictions are written as `<save_dir>/<clip:04d>_<tracker>.json` in the format
-        of `save_predictions`.  The trackers' own `results` are left untouched."""
+        of `save_predictions`.  The trackers' own `results` are left untouched.
+
+        inference_dir: each clip's annotated video is written to `<inference_dir>/<clip:04d>.mp4` (mp4v, the clip's
+        fps and frame size), the frames `TrackingRunner(trackers, video_info=<the clip's>, inference_path=...).run()`
+        writes for that clip alone.  collect_data: `clips_data_analytics` holds one `DataAnalytics` per clip, each
+        equal to that run's `data_analytics`; with `save_dir` each is also written as `<save_dir>/<clip:04d>_data.csv`
+        (`into_dataframe(<clip fps>).to_csv`).  Without `inference_dir` the positions are collected without reading
+        a frame again.  A clip of 0 frames gets no video and an empty `DataAnalytics` (no frames).  The clips are
+        rendered in one pass after the tracking pass (`_render_clips`), on rank 0 only under torch.distributed."""
         import gc
 
+        import torch.distributed as dist
+
+        srcs, lengths, fps, hw = self._clip_sources(clips)
+        saved = {n: {k: t.__dict__[k] for k in ("video_info", "byte_track") if k in t.__dict__}
+                 for n, t in self.trackers.items()}  # the per-clip stages replace these; run() finds them as they were
         gc_was_on = gc.isenabled()
         gc.disable()
         try:
-            out = self._run_clips(clips, streams)
+            out, hw = self._run_clips(srcs, lengths, fps, hw, streams)
+            rank = dist.get_rank() if dist.is_available() and dist.is_initialized() else 0
+            if rank == 0 and (inference_dir or collect_data):
+                if hw is None and lengths:  # no frame was read: (source, length) pairs, fixed detections only
+                    hw = (self.video_info.height, self.video_info.width)
+                infos = [sv.VideoInfo(width=hw[1], height=hw[0], fps=f, total_frames=T) for f, T in zip(fps, lengths)]
+                t0 = timeit.default_timer()
+                self._render_clips(srcs, infos, out, inference_dir, collect_data)
+                self.timings["_clips_render"] = timeit.default_timer() - t0
         finally:
             if gc_was_on:
                 gc.enable()
+            for n, t in self.trackers.items():
+                t.__dict__.update(saved[n])
         if save_dir is not None:
             import json
 
@@ -634,13 +666,65 @@ class TrackingRunner:
                 for name, objs in res.items():
                     with open(os.path.join(save_dir, f"{c:04d}_{name}.json"), "w") as f:
                         json.dump([o.serialize() for o in objs], f)
+            if collect_data and rank == 0:  # main.py:180-181 per clip
+                for c, da in enumerate(self.clips_data_analytics):
+                    da.into_dataframe(fps[c]).to_csv(os.path.join(save_dir, f"{c:04d}_data.csv"))
         return out
 
-    def _run_clips(self, clips: list, streams: Optional[int]) -> list[dict]:
-        import itertools
+    def _render_clips(self, srcs: list, infos: list, results: list[dict], inference_dir: Optional[str],
+                      collect_data: bool) -> None:
+        """The drawing pass of `draw_and_collect_data` over the clips played back to back: one `OverlayRenderer` (one
+        set of pinned buffers, one sprite cache), batches that cross clip boundaries (`plan_clip_render`), each frame
+        drawn from its clip's results, video_info, homography state and `DataAnalytics`, and one writer thread per
+        clip (`write_clip_batches`)."""
+        import queue
 
-        from .ball_tracker import median_background_device
+        from ..render import DisplayListBuilder, OverlayRenderer, VideoWriterThread, plan_clip_render, \
+            write_clip_batches
 
+        lengths = [int(vi.total_frames) for vi in infos]
+        das = [DataAnalytics() for _ in lengths] if collect_data else None
+        court = ProjectedCourt(infos[0]) if infos else None
+        if not inference_dir:  # data only: the positions need no frame
+            for c, T in enumerate(lengths):
+                self._collect_positions(results[c], T, court, das[c])
+        elif sum(lengths):
+            os.makedirs(inference_dir, exist_ok=True)
+            hw = (infos[0].height, infos[0].width)
+            B = self.render_batch_size
+            plan = plan_clip_render(lengths, B)
+            builder = DisplayListBuilder(hw, court)
+            renderer = OverlayRenderer(hw, B, builder.lut, out_slots=3)
+
+            def build(first, n):
+                recs = []
+                for c, f in plan[first // B].rows:
+                    if f == 0:  # every clip starts as a run() of its own would
+                        court.H = None
+                        for t in self.trackers.values():
+                            t.video_info_post_init(infos[c])
+                    recs.append(builder.frame_records(f, self.trackers, das[c] if das else None,
+                                                      self.is_fixed_keypoints, results[c]))
+                return recs
+
+            def open_writer(c, release):
+                return VideoWriterThread(os.path.join(inference_dir, f"{c:04d}.mp4"), infos[c].fps,
+                                         infos[c].resolution_wh, release)
+
+            free = queue.Queue()
+            for slot in range(3):
+                free.put(slot)
+            batches = renderer.run(_clip_render_batches(srcs, lengths, B, hw), build, free)
+            self.timings["_clips_render_encode"] = write_clip_batches(plan, batches, open_writer, free)
+            for k, v in renderer.times.items():
+                self.timings[f"_clips_render_{k}"] = v
+        if das is not None:
+            for da in das:  # q7, per clip
+                da.frames = da.frames[:-1]
+            self.clips_data_analytics = das
+
+    def _clip_sources(self, clips: list):
+        """(frame sources, lengths, fps, frame size or None when only the frames can tell) of the clips."""
         srcs, lengths, fps, hw = [], [], [], None
         for i, clip in enumerate(clips):
             if isinstance(clip, (str, os.PathLike)):
@@ -663,6 +747,14 @@ class TrackingRunner:
                 fps.append(self.video_info.fps)
         if any(t < 0 for t in lengths):
             raise ValueError("clip lengths must be >= 0")
+        return srcs, lengths, fps, hw
+
+    def _run_clips(self, srcs: list, lengths: list[int], fps: list, hw, streams: Optional[int]):
+        """The tracking pass of run_clips -> (per-clip results, frame size or None when no frame was read)."""
+        import itertools
+
+        from .ball_tracker import median_background_device
+
         fixed = {n: t for n, t in self.trackers.items() if getattr(t, "fixed_keypoints_detection", None) is not None}
         model = {n: t for n, t in self.trackers.items() if n not in fixed and (
             isinstance(t, (PlayerTracker, PlayerKeypointsTracker, BallTracker)) or
@@ -674,7 +766,7 @@ class TrackingRunner:
         if not model or not sum(lengths):
             for res, T in zip(out, lengths):
                 res.update({n: [] for n in model})
-            return out
+            return out, hw
         ball_name, ball = next(((n, t) for n, t in model.items() if isinstance(t, BallTracker)), (None, None))
         B = min(t.batch_size for t in model.values())
         side = torch.cuda.Stream()  # backgrounds of the clips ahead are computed beside the pass
@@ -761,8 +853,6 @@ class TrackingRunner:
                     pieces.append(pinned[k % 3][run0:n])
                 yield pieces
 
-        saved = {n: {k: t.__dict__[k] for k in ("video_info", "byte_track") if k in t.__dict__}
-                 for n, t in model.items()}  # the per-clip stages below replace these; run() finds them as they were
         for t in model.values():
             t.to(t.DEVICE)
         t0 = timeit.default_timer()
@@ -803,11 +893,10 @@ class TrackingRunner:
         for name, per_clip in yolo.items():
             for c, objs in enumerate(per_clip):
                 out[c][name] = objs
-        for n, t in model.items():
-            t.__dict__.update(saved[n])
+        for t in model.values():
             t.to("cpu")
         self.timings["_clips_pass"] = timeit.default_timer() - t0
-        return [{n: res[n] for n in self.trackers} for res in out]
+        return [{n: res[n] for n in self.trackers} for res in out], hw
 
 
 # ---- fixed-capacity records for the gather (SURVEY §8e) ---------------------------------------------------------
@@ -860,6 +949,38 @@ def _ball_records(xyv: dict, lo: int, hi: int) -> BallRecords:
         data[a[:, 0], :3] = a[:, 1:]
         data[a[:, 0], 3] = 1
     return BallRecords(lo, torch.from_numpy(data))
+
+
+def _clip_render_batches(srcs: list, lengths: list[int], batch_size: int, hw: tuple[int, int]) -> Iterable:
+    """The frames of the clips played back to back, re-read from their sources, in batches of `batch_size` that cross
+    clip boundaries: a device tensor when the frames are on the device, else a list of HWC host frames."""
+    buf = []
+
+    def batch():
+        if any(isinstance(f, torch.Tensor) for f in buf):
+            return torch.stack([torch.as_tensor(f, device="cuda") for f in buf])
+        return buf
+
+    for c, T in enumerate(lengths):
+        if T == 0:
+            continue
+        seen = 0
+        for item in srcs[c](0, T):
+            frames = item if getattr(item, "ndim", 3) == 4 else [item]
+            for f in frames[:T - seen]:
+                if tuple(f.shape[:2]) != hw:
+                    raise ValueError(f"clip {c} has {tuple(f.shape[:2])} frames, the first clip {hw}")
+                buf.append(f.numpy() if isinstance(f, torch.Tensor) and f.device.type != "cuda" else f)
+                seen += 1
+                if len(buf) == batch_size:
+                    yield batch()
+                    buf = []
+            if seen == T:
+                break
+        if seen != T:
+            raise ValueError(f"clip {c} yielded {seen} frames, {T} announced")
+    if buf:
+        yield batch()
 
 
 def _comm_device() -> torch.device:
