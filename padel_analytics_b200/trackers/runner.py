@@ -5,7 +5,8 @@ detections are gathered once per tracker and the sequential host stages (ByteTra
 After the trackers, `run()` renders the annotated video to `inference_path` and collects the players' court positions
 into `data_analytics` (runner.py:91-173) when either is asked for; the overlays are composited on the device
 (render.py, `pb_render_overlay`) and encoding runs on a thread of its own.  `run_clips()` does the same per clip for a
-list of clips, in one render pass over the clips played back to back.
+list of clips, in one render pass over the clips played back to back; under torch.distributed it shards whole clips
+over the ranks (`plan_clip_shards`) and exchanges the results once after the pass.
 
 Documented deviations from reference quirks (SURVEY App. E):
   q7  with collect_data=False the reference's drawing pass ends by trimming `self.data_analytics.frames`, which is
@@ -35,6 +36,26 @@ from ..analytics import DataAnalytics, ProjectedCourt
 def shard_range(total: int, rank: int, world: int) -> tuple[int, int]:
     """Contiguous frame range of `rank` (SURVEY §8e): [rank*N/R, (rank+1)*N/R)."""
     return rank * total // world, (rank + 1) * total // world
+
+
+def plan_clip_shards(lengths: list[int], world: int) -> list[list[int]]:
+    """Whole clips per rank for `run_clips` under torch.distributed: longest clip first (ties: lower clip index), each
+    to the rank with the fewest frames so far (ties: lower rank); each rank's clips in ascending order.  A pure
+    function of its arguments, so every rank computes the same plan without communicating.  Clips of 0 frames are
+    assigned too; a rank may get no clip.  The largest load is at most the mean load plus the longest clip."""
+    import heapq
+
+    if world < 1:
+        raise ValueError(f"world size must be >= 1, got {world}")
+    if any(T < 0 for T in lengths):
+        raise ValueError("clip lengths must be >= 0")
+    heap = [(0, r) for r in range(world)]  # (frames so far, rank): pops the least loaded, lowest rank first
+    shards = [[] for _ in range(world)]
+    for c in sorted(range(len(lengths)), key=lambda c: (-lengths[c], c)):
+        load, r = heapq.heappop(heap)
+        shards[r].append(c)
+        heapq.heappush(heap, (load + int(lengths[c]), r))
+    return [sorted(s) for s in shards]
 
 
 def ball_shard_frames(total: int, start: int, end: int) -> tuple[int, int]:
@@ -281,6 +302,7 @@ class TrackingRunner:
         self.render_batch_size = 32
         self.clips_data_analytics: list[DataAnalytics] = []  # per clip, filled by run_clips(collect_data=True)
         self._source = None  # (frame_source, total_frames) of the last run(), for the drawing pass
+        self._clip_reading: Optional[int] = None  # run_clips: the clip whose frames the pass read last
         self.timings: dict[str, float] = {}
 
     def restart(self) -> None:
@@ -633,23 +655,27 @@ class TrackingRunner:
         equal to that run's `data_analytics`; with `save_dir` each is also written as `<save_dir>/<clip:04d>_data.csv`
         (`into_dataframe(<clip fps>).to_csv`).  Without `inference_dir` the positions are collected without reading
         a frame again.  A clip of 0 frames gets no video and an empty `DataAnalytics` (no frames).  The clips are
-        rendered in one pass after the tracking pass (`_render_clips`), on rank 0 only under torch.distributed."""
+        rendered in one pass after the tracking pass (`_render_clips`).
+
+        Under torch.distributed (world size > 1) the clips are sharded over the ranks (`_run_clips_sharded`): each
+        rank tracks and renders only its own clips and writes only their files, and every rank returns every clip's
+        results."""
         import gc
 
         import torch.distributed as dist
 
         srcs, lengths, fps, hw = self._clip_sources(clips)
+        sharded = dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1
         saved = {n: {k: t.__dict__[k] for k in ("video_info", "byte_track") if k in t.__dict__}
                  for n, t in self.trackers.items()}  # the per-clip stages replace these; run() finds them as they were
         gc_was_on = gc.isenabled()
         gc.disable()
         try:
+            if sharded:
+                return self._run_clips_sharded(srcs, lengths, fps, hw, save_dir, streams, inference_dir, collect_data)
             out, hw = self._run_clips(srcs, lengths, fps, hw, streams)
-            rank = dist.get_rank() if dist.is_available() and dist.is_initialized() else 0
-            if rank == 0 and (inference_dir or collect_data):
-                if hw is None and lengths:  # no frame was read: (source, length) pairs, fixed detections only
-                    hw = (self.video_info.height, self.video_info.width)
-                infos = [sv.VideoInfo(width=hw[1], height=hw[0], fps=f, total_frames=T) for f, T in zip(fps, lengths)]
+            if inference_dir or collect_data:
+                infos = self._clip_infos(hw, fps, lengths)
                 t0 = timeit.default_timer()
                 self._render_clips(srcs, infos, out, inference_dir, collect_data)
                 self.timings["_clips_render"] = timeit.default_timer() - t0
@@ -659,30 +685,93 @@ class TrackingRunner:
             for n, t in self.trackers.items():
                 t.__dict__.update(saved[n])
         if save_dir is not None:
-            import json
+            self._save_clips(save_dir, range(len(out)), out, self.clips_data_analytics if collect_data else None, fps)
+        return out
 
-            os.makedirs(save_dir, exist_ok=True)
-            for c, res in enumerate(out):
-                for name, objs in res.items():
-                    with open(os.path.join(save_dir, f"{c:04d}_{name}.json"), "w") as f:
-                        json.dump([o.serialize() for o in objs], f)
-            if collect_data and rank == 0:  # main.py:180-181 per clip
-                for c, da in enumerate(self.clips_data_analytics):
-                    da.into_dataframe(fps[c]).to_csv(os.path.join(save_dir, f"{c:04d}_data.csv"))
+    def _clip_infos(self, hw, fps: list, lengths: list[int]) -> list:
+        if hw is None and lengths:  # no frame was read: (source, length) pairs, fixed detections only
+            hw = (self.video_info.height, self.video_info.width)
+        return [sv.VideoInfo(width=hw[1], height=hw[0], fps=f, total_frames=T) for f, T in zip(fps, lengths)]
+
+    @staticmethod
+    def _save_clips(save_dir: str, which: Iterable[int], results: list[dict], das: Optional[list], fps: list) -> None:
+        """Clips `which`: `<clip:04d>_<tracker>.json` (the `save_predictions` format) and, with `das`, `_data.csv`
+        (main.py:180-181 per clip)."""
+        import json
+
+        os.makedirs(save_dir, exist_ok=True)
+        for c in which:
+            for name, objs in results[c].items():
+                with open(os.path.join(save_dir, f"{c:04d}_{name}.json"), "w") as f:
+                    json.dump([o.serialize() for o in objs], f)
+            if das is not None:
+                das[c].into_dataframe(fps[c]).to_csv(os.path.join(save_dir, f"{c:04d}_data.csv"))
+
+    def _run_clips_sharded(self, srcs: list, lengths: list[int], fps: list, hw, save_dir: Optional[str],
+                           streams: Optional[int], inference_dir: Optional[str], collect_data: bool) -> list[dict]:
+        """run_clips over the ranks of a torch.distributed job.  `plan_clip_shards` gives each rank whole clips; the
+        rank runs every per-clip stage of its own clips (`_run_clips`: background, ByteTrack restart, InpaintNet) and
+        never reads another rank's clip.  After the pass the ranks exchange once: first each rank's status (its
+        error, the frame size it saw), so that a failure or a frame-size mismatch on any rank raises `ValueError` on
+        every rank instead of leaving one blocked in a collective; then every clip's results as dense arrays
+        (`exchange_clip_results`).  Each rank renders its own clips (`_render_clips`, files named by the global clip
+        index) and writes their JSON and CSV files; the ranks are assumed to share `save_dir` and `inference_dir`.
+        The render ends with a second status exchange that also carries the clips' `DataAnalytics`, so every rank's
+        `clips_data_analytics` holds every clip's, in clip order."""
+        import torch.distributed as dist
+
+        rank, world = dist.get_rank(), dist.get_world_size()
+        mine = plan_clip_shards(lengths, world)[rank]
+        own = seen = failure = cause = None
+        self._clip_reading = None
+        try:
+            own, seen = self._run_clips([srcs[c] for c in mine], [lengths[c] for c in mine], [fps[c] for c in mine],
+                                        hw, streams, clip_ids=mine)
+        except Exception as e:  # every rank must reach the status exchange
+            failure, cause = (self._clip_reading, f"{type(e).__name__}: {e}"), e
+        t0 = timeit.default_timer()
+        seen = exchange_clip_status(failure, seen, next((c for c in mine if lengths[c]), None), cause)
+        hw = hw if seen is None else seen
+        fixed = {n: t.fixed_keypoints_detection for n, t in self.trackers.items()
+                 if getattr(t, "fixed_keypoints_detection", None) is not None}
+        out = exchange_clip_results(dict(zip(mine, own)), lengths, list(self.trackers), fixed)
+        self.timings["_clips_exchange"] = timeit.default_timer() - t0
+        das = None
+        if inference_dir or collect_data:
+            infos = self._clip_infos(hw, fps, lengths)
+            failure = cause = None
+            t0 = timeit.default_timer()
+            try:
+                self._render_clips([srcs[c] for c in mine], [infos[c] for c in mine], own, inference_dir,
+                                   collect_data, clip_ids=mine)
+            except Exception as e:
+                failure, cause = (None, f"{type(e).__name__}: {e}"), e
+            self.timings["_clips_render"] = timeit.default_timer() - t0
+            t0 = timeit.default_timer()
+            own_das = dict(zip(mine, self.clips_data_analytics)) if collect_data and failure is None else {}
+            das = exchange_clip_data(failure, own_das, cause)
+            if collect_data:
+                self.clips_data_analytics = das
+            else:
+                das = None
+            self.timings["_clips_exchange"] += timeit.default_timer() - t0
+        if save_dir is not None:
+            self._save_clips(save_dir, mine, out, das, fps)
         return out
 
     def _render_clips(self, srcs: list, infos: list, results: list[dict], inference_dir: Optional[str],
-                      collect_data: bool) -> None:
+                      collect_data: bool, clip_ids: Optional[list[int]] = None) -> None:
         """The drawing pass of `draw_and_collect_data` over the clips played back to back: one `OverlayRenderer` (one
         set of pinned buffers, one sprite cache), batches that cross clip boundaries (`plan_clip_render`), each frame
         drawn from its clip's results, video_info, homography state and `DataAnalytics`, and one writer thread per
-        clip (`write_clip_batches`)."""
+        clip (`write_clip_batches`).  clip_ids: the clips' numbers in file names and messages (default 0, 1, ...)."""
         import queue
 
         from ..render import DisplayListBuilder, OverlayRenderer, VideoWriterThread, plan_clip_render, \
             write_clip_batches
 
         lengths = [int(vi.total_frames) for vi in infos]
+        ids = list(range(len(infos))) if clip_ids is None else list(clip_ids)
         das = [DataAnalytics() for _ in lengths] if collect_data else None
         court = ProjectedCourt(infos[0]) if infos else None
         if not inference_dir:  # data only: the positions need no frame
@@ -708,13 +797,13 @@ class TrackingRunner:
                 return recs
 
             def open_writer(c, release):
-                return VideoWriterThread(os.path.join(inference_dir, f"{c:04d}.mp4"), infos[c].fps,
+                return VideoWriterThread(os.path.join(inference_dir, f"{ids[c]:04d}.mp4"), infos[c].fps,
                                          infos[c].resolution_wh, release)
 
             free = queue.Queue()
             for slot in range(3):
                 free.put(slot)
-            batches = renderer.run(_clip_render_batches(srcs, lengths, B, hw), build, free)
+            batches = renderer.run(_clip_render_batches(srcs, lengths, B, hw, ids), build, free)
             self.timings["_clips_render_encode"] = write_clip_batches(plan, batches, open_writer, free)
             for k, v in renderer.times.items():
                 self.timings[f"_clips_render_{k}"] = v
@@ -749,12 +838,16 @@ class TrackingRunner:
             raise ValueError("clip lengths must be >= 0")
         return srcs, lengths, fps, hw
 
-    def _run_clips(self, srcs: list, lengths: list[int], fps: list, hw, streams: Optional[int]):
-        """The tracking pass of run_clips -> (per-clip results, frame size or None when no frame was read)."""
+    def _run_clips(self, srcs: list, lengths: list[int], fps: list, hw, streams: Optional[int],
+                   clip_ids: Optional[list[int]] = None):
+        """The tracking pass of run_clips -> (per-clip results, frame size or None when no frame was read).
+        clip_ids: the clips' numbers in messages and in `_clip_reading`, the clip whose frames were read last
+        (default 0, 1, ...)."""
         import itertools
 
         from .ball_tracker import median_background_device
 
+        ids = list(range(len(srcs))) if clip_ids is None else list(clip_ids)
         fixed = {n: t for n, t in self.trackers.items() if getattr(t, "fixed_keypoints_detection", None) is not None}
         model = {n: t for n, t in self.trackers.items() if n not in fixed and (
             isinstance(t, (PlayerTracker, PlayerKeypointsTracker, BallTracker)) or
@@ -778,6 +871,7 @@ class TrackingRunner:
 
         def items_of(c):
             """clip c's frames as (n,H,W,3) uint8 tensors, after queueing its background when it needs one"""
+            self._clip_reading = ids[c]
             it = iter(srcs[c](0, lengths[c]))
             head = []
             if ball is not None and lengths[c] >= 8:
@@ -808,7 +902,7 @@ class TrackingRunner:
                 if shape["hw"] is None:
                     shape["hw"] = tuple(t.shape[1:3])
                 if tuple(t.shape[1:3]) != shape["hw"]:
-                    raise ValueError(f"clip {c} has {tuple(t.shape[1:3])} frames, the first clip "
+                    raise ValueError(f"clip {ids[c]} has {tuple(t.shape[1:3])} frames, the first clip "
                                      f"{shape['hw']}: all clips of one call must have the same frame size")
                 t = t[:lengths[c] - seen]
                 seen += t.shape[0]
@@ -817,7 +911,7 @@ class TrackingRunner:
                 if seen == lengths[c]:
                     break
             if seen != lengths[c]:
-                raise ValueError(f"clip {c} yielded {seen} frames, {lengths[c]} announced")
+                raise ValueError(f"clip {ids[c]} yielded {seen} frames, {lengths[c]} announced")
 
         pinned = []
 
@@ -951,9 +1045,12 @@ def _ball_records(xyv: dict, lo: int, hi: int) -> BallRecords:
     return BallRecords(lo, torch.from_numpy(data))
 
 
-def _clip_render_batches(srcs: list, lengths: list[int], batch_size: int, hw: tuple[int, int]) -> Iterable:
+def _clip_render_batches(srcs: list, lengths: list[int], batch_size: int, hw: tuple[int, int],
+                         clip_ids: Optional[list[int]] = None) -> Iterable:
     """The frames of the clips played back to back, re-read from their sources, in batches of `batch_size` that cross
-    clip boundaries: a device tensor when the frames are on the device, else a list of HWC host frames."""
+    clip boundaries: a device tensor when the frames are on the device, else a list of HWC host frames.  clip_ids:
+    the clips' numbers in messages (default 0, 1, ...)."""
+    clip_ids = list(range(len(srcs))) if clip_ids is None else clip_ids
     buf = []
 
     def batch():
@@ -969,7 +1066,7 @@ def _clip_render_batches(srcs: list, lengths: list[int], batch_size: int, hw: tu
             frames = item if getattr(item, "ndim", 3) == 4 else [item]
             for f in frames[:T - seen]:
                 if tuple(f.shape[:2]) != hw:
-                    raise ValueError(f"clip {c} has {tuple(f.shape[:2])} frames, the first clip {hw}")
+                    raise ValueError(f"clip {clip_ids[c]} has {tuple(f.shape[:2])} frames, the first clip {hw}")
                 buf.append(f.numpy() if isinstance(f, torch.Tensor) and f.device.type != "cuda" else f)
                 seen += 1
                 if len(buf) == batch_size:
@@ -978,9 +1075,169 @@ def _clip_render_batches(srcs: list, lengths: list[int], batch_size: int, hw: tu
             if seen == T:
                 break
         if seen != T:
-            raise ValueError(f"clip {c} yielded {seen} frames, {T} announced")
+            raise ValueError(f"clip {clip_ids[c]} yielded {seen} frames, {T} announced")
     if buf:
         yield batch()
+
+
+# ---- run_clips over ranks: the exchange after the pass ------------------------------------------------------------
+def _all_gather(obj) -> list:
+    """Every rank's `obj`, in rank order (all_gather_object: gloo, or NCCL on the current device)."""
+    import torch.distributed as dist
+
+    out = [None] * dist.get_world_size()
+    dist.all_gather_object(out, obj)
+    return out
+
+
+def _raise_on_failure(failures: list, cause: Optional[BaseException]) -> None:
+    """failures: per rank, None or (clip or None, message).  Every rank raises the same ValueError when any failed."""
+    bad = [f"rank {r}" + ("" if f[0] is None else f", clip {f[0]}") + f": {f[1]}"
+           for r, f in enumerate(failures) if f is not None]
+    if bad:
+        raise ValueError("run_clips failed on " + "; ".join(bad)) from cause
+
+
+def exchange_clip_status(failure: Optional[tuple], hw: Optional[tuple], clip: Optional[int],
+                         cause: Optional[BaseException] = None) -> Optional[tuple]:
+    """The status exchange after a rank's tracking pass: failure = None or (clip or None, message); hw = the frame
+    size the rank saw (None if it read no frame), first at `clip`.  Every rank raises ValueError if any rank failed or
+    if two ranks saw different frame sizes; otherwise returns the frame size seen (None if no rank read a frame)."""
+    statuses = _all_gather((failure, None if hw is None else tuple(hw), clip))
+    _raise_on_failure([s[0] for s in statuses], cause)
+    sizes = [(c, h) for _, h, c in statuses if h is not None]
+    for c, h in sizes[1:]:
+        if h != sizes[0][1]:
+            raise ValueError(f"clip {c} has {h} frames, clip {sizes[0][0]} {sizes[0][1]}: all clips of one call must "
+                             "have the same frame size")
+    return sizes[0][1] if sizes else None
+
+
+def exchange_clip_results(own: dict[int, dict[str, list]], lengths: list[int], names: list[str],
+                          fixed: dict[str, object]) -> list[dict[str, list]]:
+    """Every clip's results on every rank.  own: {clip: {tracker name: list[Object]}} of this rank's clips (the
+    objects are returned as they are); every other clip's are rebuilt from the dense arrays its owner sends
+    (`_pack_objects`), `serialize()`-equal to the owner's.  fixed: {tracker name: fixed detection}, repeated per frame
+    on every rank rather than sent.  Returns one {tracker name: list[Object]} per clip, in clip order, with the
+    trackers in `names` order."""
+    packed = {c: {n: _pack_objects(objs) for n, objs in res.items() if n not in fixed} for c, res in own.items()}
+    theirs = {}
+    for part in _all_gather(packed):
+        theirs.update(part)
+    out = []
+    for c, T in enumerate(lengths):
+        if c in own:
+            out.append(own[c])
+        else:
+            out.append({n: [fixed[n]] * T if n in fixed else _unpack_objects(theirs[c][n]) for n in names})
+    return out
+
+
+def exchange_clip_data(failure: Optional[tuple], own: dict[int, DataAnalytics],
+                       cause: Optional[BaseException] = None) -> list[DataAnalytics]:
+    """The status exchange after a rank's render, carrying its clips' DataAnalytics (as `into_dict` columns).  Every
+    rank raises ValueError if any rank failed; otherwise returns the DataAnalytics of every clip any rank sent, in clip
+    order (this rank's own objects, the others rebuilt with `from_dict`: equal `frames`, `len()` and
+    `into_dataframe`)."""
+    statuses = _all_gather((failure, {c: da.into_dict() for c, da in own.items()}))
+    _raise_on_failure([s[0] for s in statuses], cause)
+    theirs = {c: d for _, part in statuses for c, d in part.items()}
+    return [own[c] if c in own else DataAnalytics.from_dict(theirs[c]) for c in sorted(theirs)]
+
+
+def _pair_is_int(xy) -> bool:
+    return isinstance(xy[0], (int, np.integer)) and isinstance(xy[1], (int, np.integer))
+
+
+def _pair(x: float, y: float, is_int: bool) -> tuple:
+    return (int(x), int(y)) if is_int else (float(x), float(y))
+
+
+def _pack_objects(objs: list) -> tuple:
+    """One clip's results of one tracker (the tracking pass's objects, which carry no projection) as (kind, per-frame
+    counts, dense per-row arrays).  Coordinates go as float64 with a per-row flag for (int, int) pairs, so the rebuilt
+    objects serialise to the same JSON, ints and floats alike."""
+    from .keypoints_tracker import Keypoints
+    from .players_keypoints_tracker import PlayerKeypoints, PlayersKeypoints
+
+    if not objs:
+        return ("empty",)
+    first = objs[0]
+    if isinstance(first, Players):
+        counts, xyxy, ids, has_id, cls, conf = [], [], [], [], [], []
+        for p in objs:
+            if p._list is None:
+                x, i, k, s = p._rows
+                n = len(x)
+                ids.append(np.zeros(n, np.int64) if i is None else np.asarray(i, np.int64))
+                has_id.append(np.full(n, i is not None))
+            else:
+                pl = p._list
+                n = len(pl)
+                x, k, s = [q.xyxy for q in pl], [q.class_id for q in pl], [q.confidence for q in pl]
+                ids.append(np.array([-1 if q.id is None else q.id for q in pl], np.int64))
+                has_id.append(np.array([q.id is not None for q in pl], bool))
+            counts.append(n)
+            xyxy.append(np.asarray(x).reshape(n, 4))
+            cls.append(np.asarray(k, np.int64).reshape(n))
+            conf.append(np.asarray(s).reshape(n))
+        return ("players", np.asarray(counts, np.int64), np.concatenate(xyxy), np.concatenate(ids),
+                np.concatenate(has_id), np.concatenate(cls), np.concatenate(conf))
+    if isinstance(first, PlayersKeypoints):
+        K = len(PlayerKeypoints.KEYPOINTS_NAMES)
+        xy = [np.asarray(p._xy if p._list is None else [[k.xy for k in pk] for pk in p._list], np.float64)
+              for p in objs]
+        xy = [a.reshape(len(a), K, 2) for a in xy]
+        return ("players_keypoints", np.asarray([len(a) for a in xy], np.int64), np.concatenate(xy))
+    if isinstance(first, Keypoints):
+        kps = [k for o in objs for k in o.keypoints]
+        return ("keypoints", np.asarray([len(o.keypoints) for o in objs], np.int64),
+                np.asarray([k.id for k in kps], np.int64).reshape(-1),
+                np.asarray([k.xy for k in kps], np.float64).reshape(-1, 2),
+                np.asarray([_pair_is_int(k.xy) for k in kps], bool).reshape(-1))
+    if isinstance(first, Ball):
+        return ("ball", np.asarray([b.frame for b in objs], np.int64), np.asarray([b.xy for b in objs], np.float64),
+                np.asarray([_pair_is_int(b.xy) for b in objs], bool), np.asarray([b.visibility for b in objs], np.int64))
+    raise TypeError(f"no dense form for {type(first).__name__} results")
+
+
+def _unpack_objects(packed: tuple) -> list:
+    """`_pack_objects` inverted: the objects, through the array-backed constructors where there are some."""
+    from .keypoints_tracker import Keypoint, Keypoints
+    from .players_keypoints_tracker import PlayersKeypoints
+    from .players_tracker import Player
+
+    kind = packed[0]
+    if kind == "empty":
+        return []
+    if kind == "ball":
+        _, frame, xy, is_int, vis = packed
+        return [Ball(frame=f, xy=_pair(x, y, i), visibility=v)
+                for f, (x, y), i, v in zip(frame.tolist(), xy.tolist(), is_int.tolist(), vis.tolist())]
+    ends = np.cumsum(packed[1]).tolist()
+    starts = [0] + ends[:-1]
+    if kind == "players":
+        _, _, xyxy, ids, has_id, cls, conf = packed
+        out = []
+        for a, b in zip(starts, ends):
+            h = has_id[a:b]
+            if h.all():
+                out.append(Players.from_rows(xyxy[a:b], ids[a:b], cls[a:b], conf[a:b]))
+            elif not h.any():
+                out.append(Players.from_rows(xyxy[a:b], None, cls[a:b], conf[a:b]))
+            else:  # ids on some players only: only a list of players holds that
+                out.append(Players([Player.from_row(xyxy[i], ids[i] if has_id[i] else None, cls[i], conf[i])
+                                    for i in range(a, b)]))
+        return out
+    if kind == "players_keypoints":
+        xy = packed[2]
+        return [PlayersKeypoints.from_xy(xy[a:b]) for a, b in zip(starts, ends)]
+    if kind == "keypoints":
+        _, _, ids, xy, is_int = packed
+        ids, xy, is_int = ids.tolist(), xy.tolist(), is_int.tolist()
+        return [Keypoints([Keypoint(id=ids[i], xy=_pair(*xy[i], is_int[i])) for i in range(a, b)])
+                for a, b in zip(starts, ends)]
+    raise ValueError(f"unknown packed kind {kind!r}")
 
 
 def _comm_device() -> torch.device:
