@@ -278,10 +278,9 @@ def render_frame_cpu(frame_bgr: np.ndarray, frame_index: int, trackers: dict, pr
 
 
 class OverlayRenderer:
-    """Batches of frames through pb_render_overlay: decoded frames are copied into pinned memory, uploaded, composited
-    and copied back into pinned buffers.  Two upload slots: while batch i is on the device, batch i+1 is decoded and
-    its display list built on the host.  Timings (seconds) accumulate in `times`: decode, build, upload, overlay,
-    download (the last three from CUDA events)."""
+    """Batches of frames through pb_render_overlay: uploaded, composited and copied back into pinned buffers.  Two
+    upload slots: while batch i is on the device, batch i+1 is read and its display list built on the host.  Timings
+    (seconds) accumulate in `times`: decode, build, upload, overlay, download (the last three from CUDA events)."""
 
     def __init__(self, frame_hw: tuple[int, int], batch_size: int, lut: np.ndarray, out_slots: int = 2):
         import torch
@@ -291,12 +290,11 @@ class OverlayRenderer:
         self.dev = torch.device("cuda")
         shape = (batch_size, H, W, 3)
         self.frames = [torch.empty(shape, dtype=torch.uint8, device=self.dev) for _ in range(2)]
-        self.pin_in = [torch.empty(shape, dtype=torch.uint8).pin_memory() for _ in range(2)]
         self.pin_out = [torch.empty(shape, dtype=torch.uint8).pin_memory() for _ in range(out_slots)]
         self.meta_host = [torch.empty(0, dtype=torch.uint8) for _ in range(2)]  # pinned: offsets | records | atlas
         self.meta_dev = [torch.empty(0, dtype=torch.uint8, device=self.dev) for _ in range(2)]
         self.lut = torch.from_numpy(np.ascontiguousarray(lut, dtype=np.uint8)).to(self.dev)
-        self.uploaded = [None, None]  # per slot: event after the last upload from its pinned buffers
+        self.uploaded = [None, None]  # per slot: event after the last upload into it
         self.times = {"decode": 0.0, "build": 0.0, "upload": 0.0, "overlay": 0.0, "download": 0.0}
         self._events = []
 
@@ -317,11 +315,13 @@ class OverlayRenderer:
         return need, o_rec, o_atl
 
     def run(self, batches: Iterable, build: Callable[[int, int], list], free_slots: Optional[queue.Queue] = None):
-        """batches: iterable of (n,H,W,3) uint8 BGR batches (numpy arrays, lists of frames, host or device tensors),
-        n <= batch_size.  build(first_frame, n) -> the batch's per-frame record lists.  Yields (frames, out_slot):
-        frames an (n,H,W,3) numpy view of pinned out-slot memory.  Without `free_slots` the out slots are used in turn
-        and a yielded batch may be overwritten as soon as the generator is advanced; with it, a slot is taken from the
-        queue before each download and the consumer puts it back when done with the frames."""
+        """batches: iterable of lists of uint8 (n,H,W,3) BGR tensors (pinned host or device) that add up to at most
+        batch_size frames (`trackers.frames.chunks`).  A batch's pieces are uploaded asynchronously: they must stay
+        untouched until the batch after next is taken.  build(first_frame, n) -> the batch's per-frame record lists.
+        Yields (frames, out_slot): frames an (n,H,W,3) numpy view of pinned out-slot memory.  Without `free_slots` the
+        out slots are used in turn and a yielded batch may be overwritten as soon as the generator is advanced; with
+        it, a slot is taken from the queue before each download and the consumer puts it back when done with the
+        frames."""
         import torch
 
         lib = L.lib()
@@ -330,22 +330,13 @@ class OverlayRenderer:
         pending, i, first = None, 0, 0
         while True:
             t0 = timeit.default_timer()
-            batch = next(it, None)
-            if batch is None:
-                break
             s = i % 2
-            if self.uploaded[s] is not None:  # the pinned buffers of this slot must have been read
+            if self.uploaded[s] is not None:  # the batch before last and this slot's metadata must have been read
                 self.uploaded[s].synchronize()
-            n = len(batch)
-            dev_src = None
-            if isinstance(batch, torch.Tensor) and batch.device.type == "cuda":
-                dev_src = batch
-            elif isinstance(batch, torch.Tensor):
-                self.pin_in[s][:n].copy_(batch)
-            else:
-                pin = self.pin_in[s].numpy()
-                for j, f in enumerate(batch):
-                    pin[j] = f
+            pieces = next(it, None)
+            if pieces is None:
+                break
+            n = sum(p.shape[0] for p in pieces)
             t1 = timeit.default_timer()
             recs, offsets, atlas = pack_display_list(build(first, n))
             nbytes, o_rec, o_atl = self._stage_meta(s, recs, offsets, atlas)
@@ -355,7 +346,10 @@ class OverlayRenderer:
             ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
             fr = self.frames[s][:n]
             ev[0].record(main)
-            fr.copy_(dev_src if dev_src is not None else self.pin_in[s][:n], non_blocking=True)
+            at = 0
+            for p in pieces:
+                fr[at:at + p.shape[0]].copy_(p, non_blocking=True)
+                at += p.shape[0]
             meta = self.meta_dev[s]
             meta[:nbytes].copy_(self.meta_host[s][:nbytes], non_blocking=True)
             ev[1].record(main)
@@ -385,25 +379,6 @@ class OverlayRenderer:
     def _finish(self, done, o: int, n: int):
         done.synchronize()
         return self.pin_out[o][:n].numpy(), o
-
-
-def frame_batches(frames: Iterable, batch_size: int) -> Iterable:
-    """Frames (HWC arrays, or ready (n,H,W,3) batches) -> batches of at most batch_size frames."""
-    chunk = []
-    for f in frames:
-        if getattr(f, "ndim", 3) == 4:
-            if chunk:
-                yield chunk
-                chunk = []
-            for a in range(0, len(f), batch_size):
-                yield f[a:a + batch_size]
-            continue
-        chunk.append(f)
-        if len(chunk) == batch_size:
-            yield chunk
-            chunk = []
-    if chunk:
-        yield chunk
 
 
 class VideoWriterThread:
@@ -537,19 +512,20 @@ def write_clip_batches(plan: list[ClipRenderBatch], batches: Iterable, open_writ
                        free_slots: queue.Queue) -> float:
     """Writes the rendered batches ((frames, out slot) pairs, in `plan` order) to one writer per clip.
     open_writer(clip, release) -> a started `VideoWriterThread` that hands slots to `release`.  Each clip's writer is
-    finished after its last part, so it drains while later clips render.  Every writer is closed before this returns;
-    the first error is raised after that.  Returns the writers' encode seconds."""
+    finished after its last part, so it drains while later clips render.  Batches that end before the plan does (a
+    source that ran short) leave the open writers with the frames they got.  Every writer is closed before this
+    returns; the first error is raised after that.  Returns the writers' encode seconds."""
     release = _SlotRelease(free_slots)
     writers: dict = {}
     error = None
     n = 0
     try:
         for frames, slot in batches:
-            b = plan[n]
-            if len(frames) != len(b.rows):
-                raise ValueError(f"render batch {n} has {len(frames)} frames, the plan {len(b.rows)}")
-            release.expect(slot, len(b.parts))
-            for p in b.parts:
+            if n == len(plan) or len(frames) > len(plan[n].rows):
+                raise ValueError(f"render batch {n} has {len(frames)} frames, more than the plan")
+            parts = [p for p in plan[n].parts if p.lo < len(frames)]
+            release.expect(slot, len(parts))
+            for p in parts:
                 if p.open:
                     if p.wait is not None:
                         writers[p.wait].closed.wait()
@@ -558,8 +534,6 @@ def write_clip_batches(plan: list[ClipRenderBatch], batches: Iterable, open_writ
                 if p.close:
                     writers[p.clip].finish()
             n += 1
-        if n != len(plan):
-            raise ValueError(f"{n} render batches, the plan has {len(plan)}")
     finally:
         for w in writers.values():
             try:

@@ -58,10 +58,10 @@ class Ball(Object):
 
 
 def median_background(frames_bgr, device="cuda") -> np.ndarray:
-    """np.median(frames_rgb, 0).astype('uint8') (iterable.py:58-81) on the device: the frames (list of HWC uint8 BGR
-    arrays, or one (T,H,W,3) uint8 tensor, host or device) are stacked in HBM and `pb_median_u8` selects the per-byte
-    median (even counts: mean of the two middle values, truncated like the reference's float64 -> uint8 cast),
-    writing RGB order.  Returns the (H,W,3) uint8 RGB median on the host."""
+    """np.median(frames_rgb, 0).astype('uint8') (iterable.py:58-81) on the device: the frames (a list of HWC uint8 BGR
+    frames or (n,H,W,3) uint8 pieces, numpy or torch, host or device) are copied piece by piece into one stack in HBM
+    and `pb_median_u8` selects the per-byte median (even counts: mean of the two middle values, truncated like the
+    reference's float64 -> uint8 cast), writing RGB order.  Returns the (H,W,3) uint8 RGB median on the host."""
     return median_background_device(frames_bgr, device).cpu().numpy()
 
 
@@ -70,18 +70,17 @@ def median_background_device(frames_bgr, device="cuda") -> torch.Tensor:
     current stream."""
     from .. import _lib as L
 
-    if isinstance(frames_bgr, torch.Tensor):
-        stack = frames_bgr.to(device).contiguous()
-    else:
-        n = len(frames_bgr)
-        H, W, _ = frames_bgr[0].shape
-        stack = torch.empty((n, H, W, 3), dtype=torch.uint8, device=device)
-        step = max(1, (256 << 20) // (H * W * 3))  # upload in ~256 MB pieces
-        for i in range(0, n, step):
-            stack[i:i + step].copy_(torch.from_numpy(np.stack(frames_bgr[i:i + step])))
-    if stack.dtype != torch.uint8 or stack.dim() != 4 or stack.shape[-1] != 3:
+    pieces = [p if isinstance(p, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(p)) for p in frames_bgr]
+    pieces = [p.unsqueeze(0) if p.dim() == 3 else p for p in pieces]
+    if any(p.dtype != torch.uint8 or p.dim() != 4 or p.shape[1:] != pieces[0].shape[1:] or p.shape[-1] != 3
+           for p in pieces):
         raise L.PbError("median_background: frames must be uint8 (T,H,W,3)")
-    T, H, W, _ = stack.shape
+    T, H, W, _ = sum(p.shape[0] for p in pieces), *pieces[0].shape[1:]
+    stack = torch.empty((T, H, W, 3), dtype=torch.uint8, device=device)
+    at = 0
+    for p in pieces:
+        stack[at:at + p.shape[0]].copy_(p)
+        at += p.shape[0]
     out = torch.empty((H, W, 3), dtype=torch.uint8, device=stack.device)
     L.check(L.lib().pb_median_u8(stack.data_ptr(), T, H * W * 3, out.data_ptr(), 1, L.stream_ptr()))
     return out

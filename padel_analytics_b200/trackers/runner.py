@@ -2,11 +2,13 @@
 multi-GPU sharded variant (SURVEY §8e): one process per GPU, contiguous frame ranges, no per-batch collectives —
 detections are gathered once per tracker and the sequential host stages (ByteTrack ids, JSON) run on rank 0.
 
-After the trackers, `run()` renders the annotated video to `inference_path` and collects the players' court positions
-into `data_analytics` (runner.py:91-173) when either is asked for; the overlays are composited on the device
-(render.py, `pb_render_overlay`) and encoding runs on a thread of its own.  `run_clips()` does the same per clip for a
-list of clips, in one render pass over the clips played back to back; under torch.distributed it shards whole clips
-over the ranks (`plan_clip_shards`) and exchanges the results once after the pass.
+Every pass reads its frame sources through `frames.py` (`read`, `chunks`, `head`).  After the trackers, `run()`
+renders the annotated video to `inference_path` and collects the players' court positions into `data_analytics`
+(runner.py:91-173) when either is asked for; the overlays are composited on the device (render.py,
+`pb_render_overlay`) and encoding runs on a thread of its own.  `run_clips()` does the same per clip for a list of
+clips.  Both draw through one render pass over clips played back to back (`_render_clips`; `run()`'s video is one
+clip).  Under torch.distributed `run_clips()` shards whole clips over the ranks (`plan_clip_shards`) and exchanges the
+results once after the pass.
 
 Documented deviations from reference quirks (SURVEY App. E):
   q7  with collect_data=False the reference's drawing pass ends by trimming `self.data_analytics.frames`, which is
@@ -16,13 +18,16 @@ Documented deviations from reference quirks (SURVEY App. E):
 """
 from __future__ import annotations
 
-import timeit
+import contextlib
+import itertools
 import os
+import timeit
 from typing import Callable, Iterable, Optional
 
 import numpy as np
 import torch
 
+from . import frames
 from . import sv_compat as sv
 from ..engine.yolo_engine import ResultBlock
 from .ball_tracker import Ball, BallTracker
@@ -104,16 +109,24 @@ class FusedPass:
             if isinstance(t, BallTracker):
                 t.stream_begin(self.hw, total_frames, first_frame, emit_range, median=median)
 
-    def _upload(self, frames, slot: int) -> torch.Tensor:
-        if not isinstance(frames, torch.Tensor):
-            frames = torch.from_numpy(np.stack(frames))
-        n = frames.shape[0]
-        if frames.device.type == "cuda":
-            return frames
+    def _upload(self, pieces, slot: int) -> torch.Tensor:
+        """pieces: uint8 (n,H,W,3) tensors (pinned host or device) that make up one batch, in order, or one such
+        tensor.  A batch of one device tensor is read in place; any other is gathered into the staging slot."""
+        if isinstance(pieces, torch.Tensor):
+            pieces = [pieces]
+        if len(pieces) == 1 and pieces[0].device.type == "cuda":
+            return pieces[0]
+        n = sum(p.shape[0] for p in pieces)
+        main = torch.cuda.current_stream()
         with torch.cuda.stream(self.copy_stream):
             if self.consumed[slot] is not None:  # the batch that last used this slot must have been read
                 self.copy_stream.wait_event(self.consumed[slot])
-            self.staging[slot][:n].copy_(frames, non_blocking=True)
+            if any(p.device.type == "cuda" for p in pieces):
+                self.copy_stream.wait_stream(main)
+            at = 0
+            for p in pieces:
+                self.staging[slot][at:at + p.shape[0]].copy_(p, non_blocking=True)
+                at += p.shape[0]
             self.ready[slot].record(self.copy_stream)
         return self.staging[slot][:n]
 
@@ -169,18 +182,18 @@ class FusedPass:
         return out
 
     def run(self, batches: Iterable):
-        """batches: iterable of uint8 (n,H,W,3) BGR batches (pinned host tensors, device tensors or lists of frames),
-        n <= batch_size.  Yields one {tracker name: results} dict per batch.
+        """batches: iterable of uint8 (n,H,W,3) BGR batches, n <= batch_size, each a pinned host or device tensor or a
+        list of such pieces (`frames.chunks`).  Yields one {tracker name: results} dict per batch.
 
         One batch of look-ahead: batch i+1 is pulled from `batches` and enqueued before batch i's results are yielded.
-        A batch (pinned host tensor: copied asynchronously into a staging slot; device tensor: read in place) must stay
+        A batch (host pieces: copied asynchronously into a staging slot; one device tensor: read in place) must stay
         untouched until ITS OWN results have been yielded, i.e. a producer that reuses buffers needs at least two."""
         it = iter(batches)
         main = torch.cuda.current_stream()
 
-        def start(frames, i):
+        def start(batch, i):
             """upload (copy stream) + enqueue all device work of batch i; returns the launch record"""
-            dev = self._upload(frames, i % 2)
+            dev = self._upload(batch, i % 2)
             staged = dev.data_ptr() == self.staging[i % 2].data_ptr()
             if staged:
                 main.wait_event(self.ready[i % 2])
@@ -230,26 +243,6 @@ class ClipPass(FusedPass):
                 pipe = t.clip_pipeline(self.hw)
                 plan = plan_clip_batches(self.lengths, t.batch_size, chunk=self.B, ring=pipe.ring, pool=pipe.pool)
                 t.clips_begin(self.hw, plan, self.median_of)
-
-    def _upload(self, pieces, slot: int) -> torch.Tensor:
-        """pieces: uint8 (n,H,W,3) tensors (pinned host or device) that make up one chunk, in order."""
-        if isinstance(pieces, torch.Tensor):
-            pieces = [pieces]
-        if len(pieces) == 1 and pieces[0].device.type == "cuda":
-            return pieces[0]
-        n = sum(p.shape[0] for p in pieces)
-        main = torch.cuda.current_stream()
-        with torch.cuda.stream(self.copy_stream):
-            if self.consumed[slot] is not None:
-                self.copy_stream.wait_event(self.consumed[slot])
-            if any(p.device.type == "cuda" for p in pieces):
-                self.copy_stream.wait_stream(main)
-            at = 0
-            for p in pieces:
-                self.staging[slot][at:at + p.shape[0]].copy_(p, non_blocking=True)
-                at += p.shape[0]
-            self.ready[slot].record(self.copy_stream)
-        return self.staging[slot][:n]
 
     def _finish(self, launched) -> dict:
         pending, nfr = launched
@@ -301,7 +294,7 @@ class TrackingRunner:
         self.data_analytics = DataAnalytics() if collect_data else None
         self.render_batch_size = 32
         self.clips_data_analytics: list[DataAnalytics] = []  # per clip, filled by run_clips(collect_data=True)
-        self._source = None  # (frame_source, total_frames) of the last run(), for the drawing pass
+        self._source = None  # frame_source of the last run(), for the drawing pass
         self._clip_reading: Optional[int] = None  # run_clips: the clip whose frames the pass read last
         self.timings: dict[str, float] = {}
 
@@ -353,7 +346,7 @@ class TrackingRunner:
 
         src = frame_source or self._frames
         total = total_frames if total_frames is not None else self.total_frames
-        self._source = (src, total)
+        self._source = src
         dist_on = dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1
         rank, world = (dist.get_rank(), dist.get_world_size()) if dist_on else (0, 1)
         lo, hi = shard_range(total, rank, world)
@@ -392,38 +385,29 @@ class TrackingRunner:
         return self.timings
 
     # ---- drawing pass (runner.py:91-173) -----------------------------------------------------------------------
-    def _render_source(self, frame_source):
-        if frame_source is not None:
-            return frame_source, len(next(iter(self.trackers.values())).results)
-        if self._source is not None:
-            return self._source
-        return self._frames, self.total_frames
-
-    def _render_batches(self, frame_source, data_analytics, free_slots=None, renderer=None):
-        """(renderer, iterator over (frames, out_slot) batches) of the whole video, overlays composited."""
-        from ..render import DisplayListBuilder, OverlayRenderer, frame_batches
-
-        if self.projected_court is None:
+    def _as_clip(self, frame_source) -> tuple[list, list, list]:
+        """The run's video as the one clip of a drawing pass: ([frame source], [video_info], [results]), the clip as
+        long as the trackers' results (the frames drawn are fewer if the source ends first)."""
+        if self.video_info is None:
             raise ValueError("rendering needs video_info (the frame size of the mini court)")
-        src, total = self._render_source(frame_source)
-        self.projected_court.H = None  # every pass starts from the first frame's keypoints
-        hw = (self.video_info.height, self.video_info.width)
-        builder = DisplayListBuilder(hw, self.projected_court)
-        if renderer is None:
-            renderer = OverlayRenderer(hw, self.render_batch_size, builder.lut,
-                                       out_slots=3 if free_slots is not None else 2)
+        vi = self.video_info
+        results = {n: t.results for n, t in self.trackers.items()}
+        info = sv.VideoInfo(width=vi.width, height=vi.height, fps=vi.fps,
+                            total_frames=len(next(iter(results.values()))))
+        return [frame_source or self._source or self._frames], [info], [results]
 
-        def build(first, n):
-            return [builder.frame_records(first + j, self.trackers, data_analytics, self.is_fixed_keypoints)
-                    for j in range(n)]
-
-        def checked(batches):
-            for b in batches:
-                if tuple(b[0].shape[:2]) != hw:
-                    raise ValueError(f"frames are {tuple(b[0].shape[:2])}, video_info says {hw}")
-                yield b
-
-        return renderer, renderer.run(checked(frame_batches(src(0, total), self.render_batch_size)), build, free_slots)
+    @contextlib.contextmanager
+    def _clip_state(self):
+        """Each clip restarts the trackers' order-dependent host stages (`video_info_post_init`: PlayerTracker gets a
+        fresh ByteTrack); their `video_info` and ByteTrack are put back on exit, so a later run() finds them as they
+        were."""
+        saved = {n: {k: t.__dict__[k] for k in ("video_info", "byte_track") if k in t.__dict__}
+                 for n, t in self.trackers.items()}
+        try:
+            yield
+        finally:
+            for n, t in self.trackers.items():
+                t.__dict__.update(saved[n])
 
     def render_frames(self, frame_source: Optional[Callable[[int, int], Iterable[np.ndarray]]] = None,
                       data_analytics: Optional[DataAnalytics] = None) -> Iterable[np.ndarray]:
@@ -431,40 +415,86 @@ class TrackingRunner:
         court, projected players and ball), as uint8 BGR host frames, one per video frame.  `frame_source` is the
         callable `run()` takes (default: the one the last `run()` used, else the video).  Positions go to
         `data_analytics` when one is given.  The overlays are composited on the device in batches."""
-        _, batches = self._render_batches(frame_source, data_analytics)
-        for frames, _ in batches:
-            for f in frames:
-                yield f.copy()
+        srcs, infos, results = self._as_clip(frame_source)
+        with self._clip_state():
+            _, _, batches = self._draw_clips(srcs, infos, results, self.projected_court,
+                                             None if data_analytics is None else [data_analytics], exact=False)
+            for out, _ in batches:
+                for f in out:
+                    yield f.copy()
 
     def draw_and_collect_data(self, frame_source=None) -> None:
         """runner.py:91-173: writes the rendered video to `inference_path` (cv2.VideoWriter, mp4v, the video's fps and
         size; encoding on a writer thread, overlapping the next batch) and fills `data_analytics` when collecting."""
-        import queue
-
-        from ..render import VideoWriterThread
-
         if self.data_analytics is not None:
             self.data_analytics.restart()
-        if self.inference_path:
+        srcs, infos, results = self._as_clip(frame_source)
+        with self._clip_state():
+            self._render_clips(srcs, infos, results, self.projected_court,
+                               None if self.data_analytics is None else [self.data_analytics],
+                               [self.inference_path] if self.inference_path else None, exact=False, prefix="_render")
+
+    def _render_clips(self, srcs: list, infos: list, results: list[dict], court: ProjectedCourt,
+                      das: Optional[list[DataAnalytics]], paths: Optional[list[str]], exact: bool, prefix: str,
+                      clip_ids: Optional[list[int]] = None) -> None:
+        """The drawing pass of `_draw_clips` with clip c's video written to paths[c] (mp4v, the clip's fps and frame
+        size) by a writer thread of its own (`write_clip_batches`), the render times going to `timings` under
+        `prefix`.  paths=None: data only, the positions need no frame (`_collect_positions`).  das: one
+        `DataAnalytics` per clip or None; each ends trimmed as the reference trims its one (q7)."""
+        import queue
+
+        from ..render import VideoWriterThread, write_clip_batches
+
+        if paths is None:
+            for c, vi in enumerate(infos):
+                self._collect_positions(results[c], int(vi.total_frames), court, das[c])
+        elif sum(int(vi.total_frames) for vi in infos):
             free = queue.Queue()
             for slot in range(3):
                 free.put(slot)
-            writer = VideoWriterThread(self.inference_path, self.video_info.fps, self.video_info.resolution_wh, free)
-            try:
-                renderer, batches = self._render_batches(frame_source, self.data_analytics, free)
-                for frames, slot in batches:
-                    writer.put(frames, slot)
-            finally:
-                writer.close()
-            self.timings["_render_encode"] = writer.seconds
+            plan, renderer, batches = self._draw_clips(srcs, infos, results, court, das, exact, clip_ids, free)
+
+            def open_writer(c, release):
+                return VideoWriterThread(paths[c], infos[c].fps, infos[c].resolution_wh, release)
+
+            self.timings[f"{prefix}_encode"] = write_clip_batches(plan, batches, open_writer, free)
             for k, v in renderer.times.items():
-                self.timings[f"_render_{k}"] = v
-        else:  # data only: the positions need no frame
-            _, total = self._render_source(frame_source)
-            self._collect_positions({n: t.results for n, t in self.trackers.items()}, total, self.projected_court,
-                                    self.data_analytics)
-        if self.data_analytics is not None:  # q7: the reference trims even when it collects nothing
-            self.data_analytics.frames = self.data_analytics.frames[:-1]  # remove the extra frame
+                self.timings[f"{prefix}_{k}"] = v
+        if das is not None:
+            for da in das:  # q7: the reference trims even when it collects nothing
+                da.frames = da.frames[:-1]  # remove the extra frame
+
+    def _draw_clips(self, srcs: list, infos: list, results: list[dict], court: ProjectedCourt,
+                    das: Optional[list[DataAnalytics]], exact: bool, clip_ids: Optional[list[int]] = None,
+                    free_slots=None):
+        """The clips played back to back through one `OverlayRenderer` (one set of pinned buffers, one sprite cache)
+        in batches that cross clip boundaries (`plan_clip_render`), each clip's frames read from srcs[c]
+        (`frames.read`: exact, or ending where the source ends) and each frame drawn from its clip's results,
+        video_info, homography state and das[c].  Every clip starts as a run() of its own would; callers hold
+        `_clip_state`.  Returns (plan, renderer, iterator over the rendered (frames, out slot) batches).  clip_ids:
+        the clips' numbers in messages (default 0, 1, ...)."""
+        from ..render import DisplayListBuilder, OverlayRenderer, plan_clip_render
+
+        lengths = [int(vi.total_frames) for vi in infos]
+        hw = (infos[0].height, infos[0].width)
+        B = self.render_batch_size
+        plan = plan_clip_render(lengths, B)
+        builder = DisplayListBuilder(hw, court)
+        renderer = OverlayRenderer(hw, B, builder.lut, out_slots=3)
+
+        def build(first, n):
+            recs = []
+            for c, f in plan[first // B].rows[:n]:  # n < rows: the source ended early
+                if f == 0:
+                    court.H = None
+                    for t in self.trackers.values():
+                        t.video_info_post_init(infos[c])
+                recs.append(builder.frame_records(f, self.trackers, None if das is None else das[c],
+                                                  self.is_fixed_keypoints, results[c]))
+            return recs
+
+        batches = _clip_render_batches(srcs, lengths, B, hw, clip_ids, exact)
+        return plan, renderer, renderer.run(batches, build, free_slots)
 
     def _collect_positions(self, results: dict, total: int, court: ProjectedCourt,
                            data_analytics: DataAnalytics) -> None:
@@ -496,11 +526,7 @@ class TrackingRunner:
 
         med = None
         if rank == 0:
-            m = min(total, tracker.median_max_sample_num)
-            frames = list(src(0, m))
-            if frames and isinstance(frames[0], torch.Tensor) and frames[0].dim() == 4:  # batched source
-                frames = torch.cat([f.to("cuda") for f in frames])[:m]
-            med = median_background(frames)
+            med = median_background(list(frames.read(src, 0, min(total, tracker.median_max_sample_num))))
         if dist_on:
             dev = _comm_device()
             shape = torch.zeros(3, dtype=torch.int64, device=dev)
@@ -524,49 +550,28 @@ class TrackingRunner:
         t0 = timeit.default_timer()
         median = self._ball_median(ball, src, total, rank, dist_on) if ball is not None else None
         t_med = timeit.default_timer() - t0
-        it = iter(src(flo, fhi))
-        first = next(it, None)
+        chunks = frames.chunks(frames.read(src, flo, fhi), B)
+        first = next(chunks, None)
         parts = {n: [] for n in model}
         hw = None
         if first is not None:
-            # a frame source may yield single HWC frames (video decode) or ready uint8 (n,H,W,3) batches, n <= B
-            # (pinned host or device tensors: no per-frame host copy)
-            batched = isinstance(first, torch.Tensor) and first.dim() == 4
-            hw = tuple(first.shape[1:3]) if batched else tuple(first.shape[:2])
-            single = not dist_on
-            fp = FusedPass(model, hw, B, total_frames=total, first_frame=flo, emit_range=(lo, hi), raw=not single,
+            hw = tuple(first[0].shape[1:3])
+            fp = FusedPass(model, hw, B, total_frames=total, first_frame=flo, emit_range=(lo, hi), raw=dist_on,
                            median=median)
-            pinned = None if batched else [torch.empty((B,) + hw + (3,), dtype=torch.uint8).pin_memory() for _ in range(3)]
-
-            def batches():
-                import itertools
-
-                if batched:
-                    yield from itertools.chain([first], it)
-                    return
-                chunk_it = sampler(itertools.chain([first], it), B)
-                for i, chunk in enumerate(chunk_it):
-                    buf = pinned[i % 3]
-                    for j, f in enumerate(chunk):
-                        buf[j].copy_(torch.from_numpy(np.ascontiguousarray(f)))
-                    yield buf[:len(chunk)]
-
             pos = flo
-            for out in fp.run(batches()):
-                n = None
+            for out in fp.run(itertools.chain([first], chunks)):
                 for name, t in model.items():
                     if isinstance(t, BallTracker):
                         parts[name].append(out[name])
                     else:
                         res = out[name]
-                        n = len(res)
-                        a, b = max(lo - pos, 0), min(hi - pos, n)  # halo frames of a ball shard are dropped
+                        a, b = max(lo - pos, 0), min(hi - pos, len(res))  # halo frames of a ball shard are dropped
                         if b > a:
                             if isinstance(res, ResultBlock):
                                 parts[name].append(res[a:b])
                             else:
                                 parts[name] += res[a:b]
-                pos += n if n is not None else B
+                pos += B  # every chunk but the last holds B frames
         torch.cuda.synchronize()
         t_pass = timeit.default_timer() - t0
         t1 = timeit.default_timer()
@@ -666,24 +671,22 @@ class TrackingRunner:
 
         srcs, lengths, fps, hw = self._clip_sources(clips)
         sharded = dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1
-        saved = {n: {k: t.__dict__[k] for k in ("video_info", "byte_track") if k in t.__dict__}
-                 for n, t in self.trackers.items()}  # the per-clip stages replace these; run() finds them as they were
         gc_was_on = gc.isenabled()
         gc.disable()
         try:
-            if sharded:
-                return self._run_clips_sharded(srcs, lengths, fps, hw, save_dir, streams, inference_dir, collect_data)
-            out, hw = self._run_clips(srcs, lengths, fps, hw, streams)
-            if inference_dir or collect_data:
-                infos = self._clip_infos(hw, fps, lengths)
-                t0 = timeit.default_timer()
-                self._render_clips(srcs, infos, out, inference_dir, collect_data)
-                self.timings["_clips_render"] = timeit.default_timer() - t0
+            with self._clip_state():
+                if sharded:
+                    return self._run_clips_sharded(srcs, lengths, fps, hw, save_dir, streams, inference_dir,
+                                                   collect_data)
+                out, hw = self._run_clips(srcs, lengths, fps, hw, streams)
+                if inference_dir or collect_data:
+                    infos = self._clip_infos(hw, fps, lengths)
+                    t0 = timeit.default_timer()
+                    self._render_clip_files(srcs, infos, out, inference_dir, collect_data)
+                    self.timings["_clips_render"] = timeit.default_timer() - t0
         finally:
             if gc_was_on:
                 gc.enable()
-            for n, t in self.trackers.items():
-                t.__dict__.update(saved[n])
         if save_dir is not None:
             self._save_clips(save_dir, range(len(out)), out, self.clips_data_analytics if collect_data else None, fps)
         return out
@@ -714,10 +717,10 @@ class TrackingRunner:
         never reads another rank's clip.  After the pass the ranks exchange once: first each rank's status (its
         error, the frame size it saw), so that a failure or a frame-size mismatch on any rank raises `ValueError` on
         every rank instead of leaving one blocked in a collective; then every clip's results as dense arrays
-        (`exchange_clip_results`).  Each rank renders its own clips (`_render_clips`, files named by the global clip
-        index) and writes their JSON and CSV files; the ranks are assumed to share `save_dir` and `inference_dir`.
-        The render ends with a second status exchange that also carries the clips' `DataAnalytics`, so every rank's
-        `clips_data_analytics` holds every clip's, in clip order."""
+        (`exchange_clip_results`).  Each rank renders its own clips (`_render_clip_files`, files named by the global
+        clip index) and writes their JSON and CSV files; the ranks are assumed to share `save_dir` and
+        `inference_dir`.  The render ends with a second status exchange that also carries the clips' `DataAnalytics`,
+        so every rank's `clips_data_analytics` holds every clip's, in clip order."""
         import torch.distributed as dist
 
         rank, world = dist.get_rank(), dist.get_world_size()
@@ -742,8 +745,8 @@ class TrackingRunner:
             failure = cause = None
             t0 = timeit.default_timer()
             try:
-                self._render_clips([srcs[c] for c in mine], [infos[c] for c in mine], own, inference_dir,
-                                   collect_data, clip_ids=mine)
+                self._render_clip_files([srcs[c] for c in mine], [infos[c] for c in mine], own, inference_dir,
+                                        collect_data, clip_ids=mine)
             except Exception as e:
                 failure, cause = (None, f"{type(e).__name__}: {e}"), e
             self.timings["_clips_render"] = timeit.default_timer() - t0
@@ -759,57 +762,21 @@ class TrackingRunner:
             self._save_clips(save_dir, mine, out, das, fps)
         return out
 
-    def _render_clips(self, srcs: list, infos: list, results: list[dict], inference_dir: Optional[str],
-                      collect_data: bool, clip_ids: Optional[list[int]] = None) -> None:
-        """The drawing pass of `draw_and_collect_data` over the clips played back to back: one `OverlayRenderer` (one
-        set of pinned buffers, one sprite cache), batches that cross clip boundaries (`plan_clip_render`), each frame
-        drawn from its clip's results, video_info, homography state and `DataAnalytics`, and one writer thread per
-        clip (`write_clip_batches`).  clip_ids: the clips' numbers in file names and messages (default 0, 1, ...)."""
-        import queue
-
-        from ..render import DisplayListBuilder, OverlayRenderer, VideoWriterThread, plan_clip_render, \
-            write_clip_batches
-
-        lengths = [int(vi.total_frames) for vi in infos]
+    def _render_clip_files(self, srcs: list, infos: list, results: list[dict], inference_dir: Optional[str],
+                           collect_data: bool, clip_ids: Optional[list[int]] = None) -> None:
+        """run_clips' drawing pass (`_render_clips`; a clip that yields fewer frames than announced raises): clip c's
+        video to `<inference_dir>/<clip id:04d>.mp4`, one `DataAnalytics` per clip into `clips_data_analytics` when
+        collecting.  clip_ids: the clips' numbers in file names and messages (default 0, 1, ...)."""
         ids = list(range(len(infos))) if clip_ids is None else list(clip_ids)
-        das = [DataAnalytics() for _ in lengths] if collect_data else None
+        paths = None
+        if inference_dir:
+            paths = [os.path.join(inference_dir, f"{c:04d}.mp4") for c in ids]
+            if any(vi.total_frames for vi in infos):
+                os.makedirs(inference_dir, exist_ok=True)
+        das = [DataAnalytics() for _ in infos] if collect_data else None
         court = ProjectedCourt(infos[0]) if infos else None
-        if not inference_dir:  # data only: the positions need no frame
-            for c, T in enumerate(lengths):
-                self._collect_positions(results[c], T, court, das[c])
-        elif sum(lengths):
-            os.makedirs(inference_dir, exist_ok=True)
-            hw = (infos[0].height, infos[0].width)
-            B = self.render_batch_size
-            plan = plan_clip_render(lengths, B)
-            builder = DisplayListBuilder(hw, court)
-            renderer = OverlayRenderer(hw, B, builder.lut, out_slots=3)
-
-            def build(first, n):
-                recs = []
-                for c, f in plan[first // B].rows:
-                    if f == 0:  # every clip starts as a run() of its own would
-                        court.H = None
-                        for t in self.trackers.values():
-                            t.video_info_post_init(infos[c])
-                    recs.append(builder.frame_records(f, self.trackers, das[c] if das else None,
-                                                      self.is_fixed_keypoints, results[c]))
-                return recs
-
-            def open_writer(c, release):
-                return VideoWriterThread(os.path.join(inference_dir, f"{ids[c]:04d}.mp4"), infos[c].fps,
-                                         infos[c].resolution_wh, release)
-
-            free = queue.Queue()
-            for slot in range(3):
-                free.put(slot)
-            batches = renderer.run(_clip_render_batches(srcs, lengths, B, hw, ids), build, free)
-            self.timings["_clips_render_encode"] = write_clip_batches(plan, batches, open_writer, free)
-            for k, v in renderer.times.items():
-                self.timings[f"_clips_render_{k}"] = v
+        self._render_clips(srcs, infos, results, court, das, paths, exact=True, prefix="_clips_render", clip_ids=ids)
         if das is not None:
-            for da in das:  # q7, per clip
-                da.frames = da.frames[:-1]
             self.clips_data_analytics = das
 
     def _clip_sources(self, clips: list):
@@ -843,8 +810,6 @@ class TrackingRunner:
         """The tracking pass of run_clips -> (per-clip results, frame size or None when no frame was read).
         clip_ids: the clips' numbers in messages and in `_clip_reading`, the clip whose frames were read last
         (default 0, 1, ...)."""
-        import itertools
-
         from .ball_tracker import median_background_device
 
         ids = list(range(len(srcs))) if clip_ids is None else list(clip_ids)
@@ -866,91 +831,31 @@ class TrackingRunner:
         meds: dict = {}
         shape = {"hw": hw}
 
-        def frame_count(item) -> int:
-            return item.shape[0] if isinstance(item, torch.Tensor) and item.dim() == 4 else 1
-
-        def items_of(c):
+        def clip_pieces(c):
             """clip c's frames as (n,H,W,3) uint8 tensors, after queueing its background when it needs one"""
             self._clip_reading = ids[c]
-            it = iter(srcs[c](0, lengths[c]))
-            head = []
+            it = frames.read(srcs[c], 0, lengths[c], shape["hw"], exact=True, clip=ids[c])
             if ball is not None and lengths[c] >= 8:
                 if ball.median is not None:
                     if "fixed" not in meds:
                         meds["fixed"] = (torch.as_tensor(ball.median).to(torch.uint8).cuda(), None)
                     meds[c] = meds["fixed"]
                 else:  # iterable.py:58-73 per clip, as TrackingRunner._ball_median does for one video
-                    m, got = min(lengths[c], ball.median_max_sample_num), 0
-                    for item in it:
-                        head.append(item)
-                        got += frame_count(item)
-                        if got >= m:
-                            break
+                    first, it = frames.head(it, min(lengths[c], ball.median_max_sample_num))
                     with torch.cuda.stream(side):
-                        if head and isinstance(head[0], torch.Tensor) and head[0].dim() == 4:
-                            med = median_background_device(torch.cat([h.to("cuda") for h in head])[:m])
-                        else:
-                            med = median_background_device([np.asarray(h) for h in head[:m]])
+                        med = median_background_device(first)
                         ready = torch.cuda.Event()
                         ready.record(side)
                     meds[c] = (med, ready)
-            seen = 0
-            for item in itertools.chain(head, it):
-                t = item if isinstance(item, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(item))
-                if t.dim() == 3:
-                    t = t.unsqueeze(0)
-                if shape["hw"] is None:
-                    shape["hw"] = tuple(t.shape[1:3])
-                if tuple(t.shape[1:3]) != shape["hw"]:
-                    raise ValueError(f"clip {ids[c]} has {tuple(t.shape[1:3])} frames, the first clip "
-                                     f"{shape['hw']}: all clips of one call must have the same frame size")
-                t = t[:lengths[c] - seen]
-                seen += t.shape[0]
-                if t.shape[0]:
-                    yield t
-                if seen == lengths[c]:
-                    break
-            if seen != lengths[c]:
-                raise ValueError(f"clip {ids[c]} yielded {seen} frames, {lengths[c]} announced")
-
-        pinned = []
-
-        def chunks():
-            """upload chunks of B frames of the concatenated clips, as lists of pieces: host frames are gathered in
-            pinned buffers (three, reused: a chunk's buffer is refilled only after its results were yielded), batch
-            tensors are passed as slices"""
-            pieces, n, k, run0 = [], 0, 0, None
-            for c in range(len(srcs)):
-                for t in items_of(c):
-                    while t.shape[0]:
-                        take = min(B - n, t.shape[0])
-                        part, t = t[:take], t[take:]
-                        if part.device.type == "cuda" or part.is_pinned():
-                            if run0 is not None:
-                                pieces.append(pinned[k % 3][run0:n])
-                                run0 = None
-                            pieces.append(part)
-                        else:
-                            if not pinned:
-                                pinned.extend(torch.empty((B,) + shape["hw"] + (3,), dtype=torch.uint8).pin_memory()
-                                              for _ in range(3))
-                            pinned[k % 3][n:n + take].copy_(part)
-                            run0 = n if run0 is None else run0
-                        n += take
-                        if n == B:
-                            if run0 is not None:
-                                pieces.append(pinned[k % 3][run0:n])
-                            yield pieces
-                            pieces, n, k, run0 = [], 0, k + 1, None
-            if n:
-                if run0 is not None:
-                    pieces.append(pinned[k % 3][run0:n])
-                yield pieces
+                    it = itertools.chain(first, it)
+            for t in it:
+                shape["hw"] = tuple(t.shape[1:3])  # the first frames read fix the size every later clip must have
+                yield t
 
         for t in model.values():
             t.to(t.DEVICE)
         t0 = timeit.default_timer()
-        gen = chunks()
+        gen = frames.chunks((t for c in range(len(srcs)) for t in clip_pieces(c)), B)
         first = next(gen)
         hw = shape["hw"]
         infos = [sv.VideoInfo(width=hw[1], height=hw[0], fps=f, total_frames=T) for f, T in zip(fps, lengths)]
@@ -1046,38 +951,13 @@ def _ball_records(xyv: dict, lo: int, hi: int) -> BallRecords:
 
 
 def _clip_render_batches(srcs: list, lengths: list[int], batch_size: int, hw: tuple[int, int],
-                         clip_ids: Optional[list[int]] = None) -> Iterable:
-    """The frames of the clips played back to back, re-read from their sources, in batches of `batch_size` that cross
-    clip boundaries: a device tensor when the frames are on the device, else a list of HWC host frames.  clip_ids:
+                         clip_ids: Optional[list[int]] = None, exact: bool = True) -> Iterable[list[torch.Tensor]]:
+    """The frames of the clips played back to back, re-read from their sources (`frames.read`: exact, or ending
+    where a source ends), in upload batches of `batch_size` that cross clip boundaries (`frames.chunks`).  clip_ids:
     the clips' numbers in messages (default 0, 1, ...)."""
-    clip_ids = list(range(len(srcs))) if clip_ids is None else clip_ids
-    buf = []
-
-    def batch():
-        if any(isinstance(f, torch.Tensor) for f in buf):
-            return torch.stack([torch.as_tensor(f, device="cuda") for f in buf])
-        return buf
-
-    for c, T in enumerate(lengths):
-        if T == 0:
-            continue
-        seen = 0
-        for item in srcs[c](0, T):
-            frames = item if getattr(item, "ndim", 3) == 4 else [item]
-            for f in frames[:T - seen]:
-                if tuple(f.shape[:2]) != hw:
-                    raise ValueError(f"clip {clip_ids[c]} has {tuple(f.shape[:2])} frames, the first clip {hw}")
-                buf.append(f.numpy() if isinstance(f, torch.Tensor) and f.device.type != "cuda" else f)
-                seen += 1
-                if len(buf) == batch_size:
-                    yield batch()
-                    buf = []
-            if seen == T:
-                break
-        if seen != T:
-            raise ValueError(f"clip {clip_ids[c]} yielded {seen} frames, {T} announced")
-    if buf:
-        yield batch()
+    ids = list(range(len(srcs))) if clip_ids is None else list(clip_ids)
+    pieces = (p for c, T in enumerate(lengths) for p in frames.read(srcs[c], 0, T, hw, exact, ids[c]))
+    return frames.chunks(pieces, batch_size)
 
 
 # ---- run_clips over ranks: the exchange after the pass ------------------------------------------------------------

@@ -7,10 +7,8 @@ import time
 
 import numpy as np
 import pytest
-import torch
 
 from padel_analytics_b200 import render as R
-from padel_analytics_b200.trackers.runner import _clip_render_batches
 
 
 def _random_lengths(rng):
@@ -125,19 +123,24 @@ def fake_encoder(monkeypatch):
     return _FakeEncoder
 
 
-def _route(plan, B, fps_of, slots=3):
+def _route(plan, B, fps_of, slots=3, frames=None):
     """Renders `plan` the way OverlayRenderer.run hands out batches (a slot is taken from the queue before each
-    batch is filled) and writes it through write_clip_batches."""
+    batch is filled) and writes it through write_clip_batches.  frames: the first `frames` rows only, as a source
+    that ends early leaves them."""
     free = queue.Queue()
     for s in range(slots):
         free.put(s)
     out = [np.full((B, 2), -1, np.int64) for _ in range(slots)]
 
     def batches():
+        left = sum(len(b.rows) for b in plan) if frames is None else frames
         for b in plan:
+            if left <= 0:
+                return
             slot = free.get(timeout=30)  # a slot that is never released fails here instead of hanging
-            buf = out[slot][:len(b.rows)]
-            buf[:] = b.rows
+            buf = out[slot][:min(len(b.rows), left)]
+            buf[:] = b.rows[:len(buf)]
+            left -= len(buf)
             yield buf, slot
 
     def open_writer(c, release):
@@ -175,19 +178,15 @@ def test_write_clip_batches_raises_a_writer_error_after_joining_every_writer(fak
     assert fake_encoder.opened["clip7"][2] == [(7, f) for f in range(30)]  # the other clips are still written
 
 
-def test_clip_render_batches_cross_clip_boundaries():
-    H, W = 4, 6
-    rng = np.random.default_rng(0)
-    clips = [rng.integers(0, 256, (T, H, W, 3), dtype=np.uint8) for T in (5, 0, 8, 9, 3)]
-    srcs = [lambda lo, hi, c=c: iter(clips[c][lo:hi]) for c in (0, 1, 2)]
-    srcs += [lambda lo, hi: (torch.from_numpy(clips[3][i:min(hi, i + 4)]) for i in range(lo, hi, 4)),
-             lambda lo, hi: iter([torch.from_numpy(clips[4])])]  # batched host tensors, one longer than the clip
-    lengths = [5, 0, 8, 9, 2]
-    got = list(_clip_render_batches(srcs, lengths, 7, (H, W)))
-    assert [len(b) for b in got] == [7, 7, 7, 3]
-    flat = np.stack([f for b in got for f in b])
-    assert np.array_equal(flat, np.concatenate([clips[0], clips[2], clips[3], clips[4][:2]]))
-    with pytest.raises(ValueError, match="announced"):
-        list(_clip_render_batches(srcs[:1], [6], 7, (H, W)))
-    with pytest.raises(ValueError, match="frames"):
-        list(_clip_render_batches(srcs[:1], [5], 7, (H + 1, W)))
+def test_write_clip_batches_ends_the_writers_where_the_frames_end(fake_encoder):
+    lengths = [5, 8, 9, 40]
+    for got in (3, 13, 16, 30, 61):
+        fake_encoder.opened = {}
+        _route(R.plan_clip_render(lengths, 8, 2), 8, lambda c: 25.0, frames=got)
+        assert fake_encoder.live == 0
+        rows = [(c, f) for c, T in enumerate(lengths) for f in range(T)][:got]
+        assert set(fake_encoder.opened) == {f"clip{c}" for c, _ in rows}  # no writer for a clip that got no frame
+        for c in {c for c, _ in rows}:
+            assert fake_encoder.opened[f"clip{c}"][2:] == [[r for r in rows if r[0] == c], True]
+    with pytest.raises(ValueError, match="more than the plan"):
+        R.write_clip_batches(R.plan_clip_render([3], 8), iter([(np.zeros((4, 2)), 0)]), None, queue.Queue())
