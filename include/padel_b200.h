@@ -186,13 +186,10 @@ int pb_pil_resize_u8(const uint8_t* src, int B, int Hs, int Ws, uint8_t* tmp, ui
 int pb_u8_to_f16_nhwc16(const uint8_t* src, int B, int H, int W, void* dst, int c0, int c1, int c2, int out_layout,
                         void* stream);
 /* TrackNet window assembly (iterable.py:167-199): frames = ring of resized RGB frames as normalised fp16 4-channel
- * pixels (ring,H,W,4) (written by pb_pil_resize_u8 with f16_layout 2), median likewise (H,W,4) ->
- * x half NHWC (B,H,W,32): channels [med(3), f[first+b+0](3) ... f[first+b+7](3), 0 x5].                          */
-int pb_tracknet_pack_windows(const void* frames, int ring, int first_slot, const void* median, int B, int H, int W,
-                             void* x, void* stream);
-/* Window assembly for a batch whose windows come from several clips: row b gathers the ring slots
- * (row_slot[b] + f) % ring, f = 0..7, and the background medians[row_median[b]] (medians: (K,H,W,4) like median).
- * row_slot, row_median: int (B) on the device.  Byte-identical to pb_tracknet_pack_windows on each row.           */
+ * pixels (ring,H,W,4) (written by pb_pil_resize_u8 with f16_layout 2), medians likewise (K,H,W,4) ->
+ * x half NHWC (B,H,W,32): row b = [medians[row_median[b]](3), frames[(row_slot[b] + 0) % ring](3) ...
+ * frames[(row_slot[b] + 7) % ring](3), 0 x5].  row_slot, row_median: int (B) on the device.  The rows of one batch
+ * may come from several clips, each with its own median.                                                          */
 int pb_tracknet_pack_windows_rows(const void* frames, int ring, const int* row_slot, const void* medians,
                                   const int* row_median, int B, int H, int W, void* x, void* stream);
 
@@ -266,17 +263,12 @@ int pb_inpaintnet_forward(const float* coor, const float* mask, int N, int L, co
 int pb_median_u8(const uint8_t* frames, int T, long long frame_bytes, uint8_t* out, int swap_rb, void* stream);
 
 /* ---- TrackNet post-processing (ball_tracker.py:449-509 ; predict.py:7-39) ---------------------------------- */
-/* Temporal ensemble + >thr. pred: float (S,8,H,W) raw heat-maps of consecutive windows; window index of pred[0]
- * is `first_window`; frames [frame0, frame0+nframes) are produced; total_windows = total_frames-7.
- * mask: u8 (nframes,H,W) (0/1). ens (optional, may be NULL): float (nframes,H,W).                               */
-int pb_tracknet_ensemble(const float* pred, int S, int first_window, int total_windows, int frame0, int nframes,
-                         int H, int W, float thr, uint8_t* mask, float* ens, void* stream);
-/* The same ensemble for frames of several clips in one launch.  pred row r holds global window first_window + r
- * (windows of consecutive clips are consecutive).  desc: int (nframes,3) on the device, per output frame
- * (global window index of its clip's first window, the clip's window count = clip frames - 7, the frame's index in
- * the clip).  Each frame uses only its clip's windows and that clip's head/tail rules: the output equals
- * pb_tracknet_ensemble run on each clip alone, bit for bit.  The caller guarantees that every window a frame needs
- * is in pred.                                                                                                     */
+/* Temporal ensemble + >thr, for frames of one or several clips in one launch.  pred: float (S,8,H,W) raw heat-maps;
+ * row r holds global window first_window + r (windows of consecutive clips are consecutive).  desc: int (nframes,3)
+ * on the device, per output frame (global window index of its clip's first window, the clip's window count = clip
+ * frames - 7, the frame's index in the clip).  Each frame uses only its clip's windows and that clip's head/tail
+ * rules.  mask: u8 (nframes,H,W) (0/1). ens (optional, may be NULL): float (nframes,H,W).  The caller guarantees
+ * that every window a frame needs is in pred.                                                                     */
 int pb_tracknet_ensemble_rows(const float* pred, int first_window, const int* desc, int nframes, int H, int W,
                               float thr, uint8_t* mask, float* ens, void* stream);
 /* 8-connected components of each mask; picks the component with max bbox area (ties: the one whose first pixel in

@@ -86,7 +86,6 @@ SIGNATURES = {
     "pb_letterbox_u8_f16": (_i, [_p, _i, _i, _i, _p, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p, _i, _i, _i, _i, _p]),
     "pb_pil_resize_u8": (_i, [_p, _i, _i, _i, _p, _p, _i, _i, _p, _p, _i, _p, _p, _i, _i, _p, _i, _p]),
     "pb_u8_to_f16_nhwc16": (_i, [_p, _i, _i, _i, _p, _i, _i, _i, _i, _p]),
-    "pb_tracknet_pack_windows": (_i, [_p, _i, _i, _p, _i, _i, _i, _p, _p]),
     "pb_tracknet_pack_windows_rows": (_i, [_p, _i, _p, _p, _p, _i, _i, _i, _p, _p]),
     "pb_yolo_decode": (_i, [C.POINTER(YoloLevel), _i, _i, _i, _i, _i, _i, _i, _i, _f, C.POINTER(C.c_int), _i, _p, _p, _p,
                              _i, _p]),
@@ -104,7 +103,6 @@ SIGNATURES = {
     "pb_bytetrack_update_many": (_i, [_p, _p, _p, _p, _i, _p]),
     "pb_inpaintnet_forward": (_i, [_p, _p, _i, _i, _p, _p, _p]),
     "pb_median_u8": (_i, [_p, _i, C.c_longlong, _p, _i, _p]),
-    "pb_tracknet_ensemble": (_i, [_p, _i, _i, _i, _i, _i, _i, _i, _f, _p, _p, _p]),
     "pb_tracknet_ensemble_rows": (_i, [_p, _i, _p, _i, _i, _i, _f, _p, _p, _p]),
     "pb_ccl_bbox": (_i, [_p, _i, _i, _i, _p, _p, _p]),
     "pb_render_overlay": (_i, [_p, _i, _i, _i, _p, _p, _p, _p, _p]),

@@ -268,48 +268,11 @@ __global__ void u8_to_f16_nhwc16_kernel(const uint8_t* __restrict__ src, long np
   }
 }
 
-// x[b, h, w, :] = [median(3), frame[first+b+0](3), ..., frame[first+b+7](3), 0*5]   (32 channels, fp16)
-// frames / median are already normalised fp16 4-channel pixels (written by the resize pass): one thread per pixel
-// gathers nine 8-byte pixels and writes one 64-byte row.
-__global__ void tracknet_pack_kernel(const uint2* __restrict__ frames, int ring, int first_slot,
-                                     const uint2* __restrict__ median, int B, int HW, uint4* __restrict__ x) {
-  const long total = (long)B * HW;
-  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-    const int pix = (int)(i % HW);
-    const int b = (int)(i / HW);
-    unsigned short h[32];
-    {
-      const uint2 m = __ldg(median + pix);
-      h[0] = (unsigned short)(m.x & 0xFFFF);
-      h[1] = (unsigned short)(m.x >> 16);
-      h[2] = (unsigned short)(m.y & 0xFFFF);
-    }
-#pragma unroll
-    for (int f = 0; f < 8; ++f) {
-      const int slot = (first_slot + b + f) % ring;
-      const uint2 p = __ldg(frames + (size_t)slot * HW + pix);
-      h[3 + 3 * f] = (unsigned short)(p.x & 0xFFFF);
-      h[4 + 3 * f] = (unsigned short)(p.x >> 16);
-      h[5 + 3 * f] = (unsigned short)(p.y & 0xFFFF);
-    }
-#pragma unroll
-    for (int j = 27; j < 32; ++j) h[j] = 0;
-    uint4* o = x + i * 4;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      uint4 v;
-      v.x = (uint32_t)h[8 * q + 0] | ((uint32_t)h[8 * q + 1] << 16);
-      v.y = (uint32_t)h[8 * q + 2] | ((uint32_t)h[8 * q + 3] << 16);
-      v.z = (uint32_t)h[8 * q + 4] | ((uint32_t)h[8 * q + 5] << 16);
-      v.w = (uint32_t)h[8 * q + 6] | ((uint32_t)h[8 * q + 7] << 16);
-      o[q] = v;
-    }
-  }
-}
-
-// The same gather, but row b takes its first ring slot from row_slot[b] and its background from
-// medians[row_median[b]]: a batch of windows that spans several clips (each clip has its own median, and the ring
-// skips the 7 frames at the end of a clip that start no window).
+// x[b, h, w, :] = [median(3), frame[slot+0](3), ..., frame[slot+7](3), 0*5]   (32 channels, fp16), where row b's
+// frames are the ring slots (row_slot[b] + f) % ring and its median is medians[row_median[b]]: a batch of windows may
+// span several clips (each clip has its own median, and the ring skips the 7 frames at the end of a clip that start no
+// window).  frames / medians are already normalised fp16 4-channel pixels (written by the resize pass): one thread per
+// pixel gathers nine 8-byte pixels and writes one 64-byte row.
 __global__ void tracknet_pack_rows_kernel(const uint2* __restrict__ frames, int ring, const int* __restrict__ row_slot,
                                           const uint2* __restrict__ medians, const int* __restrict__ row_median, int B,
                                           int HW, uint4* __restrict__ x) {
@@ -425,19 +388,6 @@ int pb_u8_to_f16_nhwc16(const uint8_t* src, int B, int H, int W, void* dst, int 
   const long npix = (long)B * H * W;
   u8_to_f16_nhwc16_kernel<<<grid_for(npix, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       src, npix, reinterpret_cast<__half*>(dst), c0, c1, c2, out_layout, H, W);
-  PB_CUDA(cudaGetLastError());
-  count_launch();
-  return 0;
-}
-
-int pb_tracknet_pack_windows(const void* frames, int ring, int first_slot, const void* median, int B, int H, int W,
-                             void* x, void* stream) {
-  PB_CHECK(frames && median && x, "tracknet_pack: null pointer");
-  PB_CHECK(ring >= 8, "tracknet_pack: ring must hold at least 8 frames");
-  const long total = (long)B * H * W;
-  tracknet_pack_kernel<<<grid_for(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      reinterpret_cast<const uint2*>(frames), ring, first_slot, reinterpret_cast<const uint2*>(median), B, H * W,
-      reinterpret_cast<uint4*>(x));
   PB_CUDA(cudaGetLastError());
   count_launch();
   return 0;

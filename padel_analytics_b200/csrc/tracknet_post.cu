@@ -8,44 +8,9 @@
 
 namespace pb {
 
-// One thread per (frame, pixel). pred holds windows [first_window, first_window+S).
-__global__ void ensemble_kernel(const float* __restrict__ pred, int S, int first_window, int total_windows,
-                                int frame0, int nframes, int HW, float thr, uint8_t* __restrict__ mask,
-                                float* __restrict__ ens) {
-  const long total = (long)nframes * HW;
-  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-    const int pix = (int)(i % HW);
-    const int n = frame0 + (int)(i / HW);  // absolute frame index
-    float acc = 0.f;
-    float result;
-    if (n < total_windows && n >= 7) {
-      // general case: sum_k w[k] * P[n-7+k][7-k], w = [1,2,3,4,4,3,2,1]/20 (products first, then summed in k order)
-#pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        const float wk = (float)(k < 4 ? k + 1 : 8 - k) / 20.0f;
-        const int s = n - 7 + k - first_window;
-        acc = __fadd_rn(acc, __fmul_rn(pred[((size_t)s * 8 + (7 - k)) * HW + pix], wk));  // mul, then add (no FMA)
-      }
-      result = acc;
-    } else {
-      // head (n < 7): mean over the n+1 windows that exist; tail (n >= total_windows): divisor 8 - frame_i
-#pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        const int w = n - 7 + k;  // absolute window
-        if (w >= 0 && w < total_windows) acc += pred[((size_t)(w - first_window) * 8 + (7 - k)) * HW + pix];
-      }
-      const float div = (n < total_windows) ? (float)(n + 1) : (float)(8 - (n - (total_windows - 1)));
-      result = acc / div;
-    }
-    mask[i] = result > thr ? 1 : 0;
-    if (ens) ens[i] = result;
-  }
-}
-
-// The same ensemble for frames of several clips in one launch.  desc[f] = (global pred row of the frame's clip's first
-// window, that clip's window count, the frame's index in its clip); pred row r holds global window first_window + r.
-// Each frame reads only its own clip's windows and applies the head/tail rules of that clip, with the arithmetic of
-// ensemble_kernel term for term.
+// One thread per (frame, pixel); the frames may belong to several clips.  desc[f] = (global window index of the
+// frame's clip's window 0, that clip's window count, the frame's index in its clip); pred row r holds global window
+// first_window + r.  Each frame reads only its own clip's windows and applies the head/tail rules of that clip.
 __global__ void ensemble_rows_kernel(const float* __restrict__ pred, int first_window, const int* __restrict__ desc,
                                      int nframes, int HW, float thr, uint8_t* __restrict__ mask,
                                      float* __restrict__ ens) {
@@ -59,14 +24,16 @@ __global__ void ensemble_rows_kernel(const float* __restrict__ pred, int first_w
     float acc = 0.f;
     float result;
     if (n < total_windows && n >= 7) {
+      // general case: sum_k w[k] * P[n-7+k][7-k], w = [1,2,3,4,4,3,2,1]/20 (products first, then summed in k order)
 #pragma unroll
       for (int k = 0; k < 8; ++k) {
         const float wk = (float)(k < 4 ? k + 1 : 8 - k) / 20.0f;
         const int s = base + n - 7 + k;
-        acc = __fadd_rn(acc, __fmul_rn(pred[((size_t)s * 8 + (7 - k)) * HW + pix], wk));
+        acc = __fadd_rn(acc, __fmul_rn(pred[((size_t)s * 8 + (7 - k)) * HW + pix], wk));  // mul, then add (no FMA)
       }
       result = acc;
     } else {
+      // head (n < 7): mean over the n+1 windows that exist; tail (n >= total_windows): divisor 8 - frame_i
 #pragma unroll
       for (int k = 0; k < 8; ++k) {
         const int w = n - 7 + k;
@@ -201,28 +168,6 @@ __global__ void __launch_bounds__(1024) ccl_bbox_kernel(const uint8_t* __restric
 using namespace pb;
 
 extern "C" {
-
-int pb_tracknet_ensemble(const float* pred, int S, int first_window, int total_windows, int frame0, int nframes,
-                         int H, int W, float thr, uint8_t* mask, float* ens, void* stream) {
-  PB_CHECK(pred && mask, "ensemble: null pointer");
-  if (nframes <= 0) return 0;
-  // every window a produced frame touches must be inside [first_window, first_window+S)
-  for (int n = frame0; n < frame0 + nframes; n += (nframes > 1 ? nframes - 1 : 1)) {
-    int lo = n - 7 < 0 ? 0 : n - 7;
-    int hi = n < total_windows - 1 ? n : total_windows - 1;
-    PB_CHECK(lo >= first_window && hi < first_window + S,
-             "ensemble: frame %d needs windows [%d,%d], buffer holds [%d,%d)", n, lo, hi, first_window,
-             first_window + S);
-  }
-  const long total = (long)nframes * H * W;
-  long blocks = (total + 255) / 256;
-  if (blocks > (long)num_sms() * 32) blocks = (long)num_sms() * 32;
-  ensemble_kernel<<<(int)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      pred, S, first_window, total_windows, frame0, nframes, H * W, thr, mask, ens);
-  PB_CUDA(cudaGetLastError());
-  count_launch();
-  return 0;
-}
 
 int pb_tracknet_ensemble_rows(const float* pred, int first_window, const int* desc, int nframes, int H, int W,
                               float thr, uint8_t* mask, float* ens, void* stream) {

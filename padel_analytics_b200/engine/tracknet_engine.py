@@ -171,38 +171,43 @@ class TrackNetEngine:
 class BallPipeline:
     """Frames (BGR u8) -> per-frame ball bbox, entirely on device: PIL-exact resize, window packing, TrackNet,
     temporal ensemble + threshold, connected components.  Mirrors BallTracker.predict_frames' TrackNet stage
-    (ball_tracker.py:373-523) including its head/tail ensemble rules (SURVEY App. C)."""
+    (ball_tracker.py:373-523) including its head/tail ensemble rules (SURVEY App. C).  One video: its background is
+    slot 0 of a one-slot median pool, and its windows are numbered from 0 as the one clip of the batch tables."""
 
     def __init__(self, engine: TrackNetEngine, frame_hw: tuple[int, int], median_rgb: np.ndarray | torch.Tensor):
-        self._init_resize(engine, frame_hw)
-        B, H, W = self.B, engine.H, engine.W
-        self.ring = B + 8
-        # resized RGB frames as normalised fp16 4-channel pixels (what the window-packing kernel gathers from)
-        self.small = torch.zeros((self.ring, H, W, 4), dtype=torch.float16, device=self.dev)
-        self.tmp = torch.zeros((B + 7, self.Hs, W, 3), dtype=torch.uint8, device=self.dev)
-        self.stage = torch.zeros((B + 7, self.Hs, self.Ws, 3), dtype=torch.uint8, device=self.dev)
-        self.mask = torch.zeros((B + 7, H, W), dtype=torch.uint8, device=self.dev)
-        self.scratch = torch.zeros((B + 7, 5, H * W), dtype=torch.int32, device=self.dev)
-        self.bbox = torch.zeros((B + 7, 4), dtype=torch.int32, device=self.dev)
-        self._host_ring = [torch.zeros((B + 7, 4), dtype=torch.int32).pin_memory() for _ in range(3)]
-        self._pending = [None] * 3
-        self._turn = 0
+        self._init_buffers(engine, frame_hw, ring=engine.B + 8, pool=1, max_frames=engine.B + 7)
+        self.stage = torch.zeros((self.B + 7, self.Hs, self.Ws, 3), dtype=torch.uint8, device=self.dev)
         self.ens = None
-        self.median_small = torch.zeros((1, H, W, 4), dtype=torch.float16, device=self.dev)
         self._median_src = None
         self.set_median(median_rgb)
         self.reset()
 
-    def _init_resize(self, engine: TrackNetEngine, frame_hw):
-        """Engine, frame size and the Pillow bicubic tables (frame size -> network size) on the device."""
+    def _init_buffers(self, engine: TrackNetEngine, frame_hw, ring: int, pool: int, max_frames: int):
+        """Pillow bicubic tables (frame size -> network size), the ring of `ring` resized frames, a pool of `pool`
+        backgrounds, and the per-batch buffers for up to `max_frames` emitted frames."""
         self.eng = engine
         self.dev = engine.device
         self.Hs, self.Ws = frame_hw
-        self.B = engine.B
-        bh, kh, self.ksh = resample.pil_bicubic_tables(self.Ws, engine.W)
-        bv, kv, self.ksv = resample.pil_bicubic_tables(self.Hs, engine.H)
+        B, H, W = engine.B, engine.H, engine.W
+        self.B, self.ring, self.pool, self.max_frames = B, ring, pool, max_frames
+        bh, kh, self.ksh = resample.pil_bicubic_tables(self.Ws, W)
+        bv, kv, self.ksv = resample.pil_bicubic_tables(self.Hs, H)
         up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(self.dev)
         self.bh, self.kh, self.bv, self.kv = up(bh), up(kh), up(bv), up(kv)
+        # resized RGB frames and backgrounds as normalised fp16 4-channel pixels (what the window-packing kernel gathers)
+        self.small = torch.zeros((ring, H, W, 4), dtype=torch.float16, device=self.dev)
+        self.medians = torch.zeros((pool, H, W, 4), dtype=torch.float16, device=self.dev)
+        self.tmp = torch.zeros((B + 7, self.Hs, W, 3), dtype=torch.uint8, device=self.dev)
+        self.mask = torch.zeros((max_frames, H, W), dtype=torch.uint8, device=self.dev)
+        self.scratch = torch.zeros((B + 7, 5, H * W), dtype=torch.int32, device=self.dev)  # boxes run B+7 at a time
+        self.bbox = torch.zeros((max_frames, 4), dtype=torch.int32, device=self.dev)
+        # a batch's tables on the device: row ring slots (B), row median slots (B), frame descriptors (max_frames, 3)
+        self._tables = torch.zeros(2 * B + 3 * max_frames, dtype=torch.int32, device=self.dev)
+        # per launch slot, pinned: the staged tables and the downloaded boxes (see _launch_batch for the slot rule)
+        self._stage = [torch.zeros(self._tables.shape, dtype=torch.int32).pin_memory() for _ in range(4)]
+        self._host_ring = [torch.zeros((max_frames, 4), dtype=torch.int32).pin_memory() for _ in range(4)]
+        self._pending = [None] * 4
+        self._turn = 0
 
     def set_median(self, median_rgb):
         """(Re)apply the background: full-res RGB -> uint8 -> PIL resize (iterable.py:76-81), on device with the same
@@ -216,7 +221,7 @@ class BallPipeline:
             return
         self._median_src = med.cpu().clone()
         dev_med = med.to(self.dev).contiguous().view(1, self.Hs, self.Ws, 3)
-        self._resize(dev_med, 1, self.median_small, swap_rb=0)
+        self._resize(dev_med, 1, self.medians[:1], swap_rb=0)
 
     def reset(self, base: int = 0):
         """base = absolute index of the first frame that will be pushed (= first window computed); > 0 for shards
@@ -262,95 +267,120 @@ class BallPipeline:
     def run_windows_async(self, nb: int, total_frames: int, want_ens: bool = False):
         """Enqueue the device work for the next nb windows; returns a callable that waits and yields
         (first_frame, bboxes).  One call in flight."""
-        eng = self.eng
         assert 0 < nb <= self.B and nb <= self.windows_ready()
         w0 = self.base + self.n_windows  # absolute window index
         total_windows = total_frames - 7
         if w0 + nb > total_windows:
             raise L.PbError("BallPipeline: more windows than total_frames allows")
-        L.check(L.lib().pb_tracknet_pack_windows(self.small.data_ptr(), self.ring, self.n_windows % self.ring,
-                                                 self.median_small.data_ptr(), nb, eng.H, eng.W, eng.x.data_ptr(),
-                                                 L.stream_ptr()))
-        eng.run_packed()
         nframes = nb + (7 if w0 + nb == total_windows else 0)
-        ens_ptr = 0
+        desc = np.zeros((nframes, 3), dtype=np.int32)  # the video is one clip whose window 0 is window 0
+        desc[:, 1] = total_windows
+        desc[:, 2] = np.arange(w0, w0 + nframes)
+        fin = self._launch_batch(w0, w0, (self.n_windows + np.arange(nb)) % self.ring, np.zeros(nb), desc, want_ens)
+        self.n_windows += nb
+        return fin
+
+    def run_ready_async(self, total_frames: int) -> list:
+        """Enqueue every window that has become computable, in batches of up to B, with at most one launch in flight
+        (each launch is waited for before the next is enqueued).  Returns the launches' finish callables in order."""
+        fins = []
+        while True:
+            nb = min(self.B, self.windows_ready(), total_frames - 7 - (self.base + self.n_windows))
+            if nb <= 0:
+                return fins
+            if fins:
+                res = fins[-1]()
+                fins[-1] = lambda res=res: res
+            fins.append(self.run_windows_async(nb, total_frames))
+
+    def _launch_batch(self, key, first_window: int, row_slot, row_median, desc, want_ens: bool = False):
+        """Enqueue one batch of nb = len(row_slot) windows: pack, TrackNet, ensemble + threshold, boxes, download.
+        Row b is global window first_window + b; it gathers the ring slots (row_slot[b] + f) % ring, f = 0..7, and
+        median pool slot row_median[b].  desc: per emitted frame, (global index of its clip's window 0, the clip's
+        window count, the frame's index in its clip).  Returns a callable that waits and yields (key, host int32
+        (nframes, 4) boxes)."""
+        eng = self.eng
+        nb = len(row_slot)
+        desc = np.asarray(desc, dtype=np.int32).reshape(-1, 3)
+        nframes = desc.shape[0]
+        # pred holds the 7 windows carried from the batch before and this batch's: [first_window - 7, first_window + nb)
+        lo = desc[:, 0] + np.maximum(desc[:, 2] - 7, 0)
+        hi = desc[:, 0] + np.minimum(desc[:, 2], desc[:, 1] - 1)
+        bad = np.flatnonzero((lo < first_window - 7) | (hi >= first_window + nb))
+        if bad.size:
+            i = bad[0]
+            raise L.PbError(f"ensemble: frame {desc[i, 2]} needs windows [{lo[i]},{hi[i]}], the buffer holds "
+                            f"[{first_window - 7},{first_window + nb})")
+        # The slot's staged tables and host boxes are rewritten only once its previous launch has completed.  That
+        # launch was waited for at the end of the launch before this one, unless that launch raised midway.
+        slot = self._turn
+        self._turn = (slot + 1) % len(self._pending)
+        if self._pending[slot] is not None:
+            self._pending[slot]()
+        stage = self._stage[slot]
+        n = 2 * nb + 3 * nframes
+        t = stage.numpy()
+        t[:nb], t[nb:2 * nb], t[2 * nb:n] = row_slot, row_median, desc.reshape(-1)
+        self._tables[:n].copy_(stage[:n], non_blocking=True)
+        rows = self._tables.data_ptr()
+        L.check(L.lib().pb_tracknet_pack_windows_rows(self.small.data_ptr(), self.ring, rows, self.medians.data_ptr(),
+                                                      rows + 4 * nb, nb, eng.H, eng.W, eng.x.data_ptr(),
+                                                      L.stream_ptr()))
+        eng.run_packed()
+        ens_ptr = None
         if want_ens:
             self.ens = torch.empty((nframes, eng.H, eng.W), dtype=torch.float32, device=self.dev)
             ens_ptr = self.ens.data_ptr()
-        L.check(L.lib().pb_tracknet_ensemble(eng.pred.data_ptr(), 7 + nb, w0 - 7, total_windows, w0, nframes, eng.H,
-                                             eng.W, 0.5, self.mask.data_ptr(), ens_ptr, L.stream_ptr()))
-        L.check(L.lib().pb_ccl_bbox(self.mask.data_ptr(), nframes, eng.H, eng.W, self.scratch.data_ptr(),
-                                    self.bbox.data_ptr(), L.stream_ptr()))
-        slot = self._turn  # ring of pinned host copies: the caller may enqueue the next batch before collecting this one
-        self._turn = (slot + 1) % len(self._host_ring)
-        if self._pending[slot] is not None:
-            self._pending[slot]()  # an uncollected launch still owns this slot: resolve it first
-        host = self._host_ring[slot]
-        host[:nframes].copy_(self.bbox[:nframes], non_blocking=True)
-        # carry the last 7 windows for the next batch (ball_tracker.py:523)
+        L.check(L.lib().pb_tracknet_ensemble_rows(eng.pred.data_ptr(), first_window - 7, rows + 8 * nb, nframes, eng.H,
+                                                  eng.W, 0.5, self.mask.data_ptr(), ens_ptr, L.stream_ptr()))
+        step = self.scratch.shape[0]
+        for f in range(0, nframes, step):  # the scratch holds B+7 frames: several launches for the short-clip case
+            m = min(step, nframes - f)
+            L.check(L.lib().pb_ccl_bbox(self.mask[f:].data_ptr(), m, eng.H, eng.W, self.scratch.data_ptr(),
+                                        self.bbox[f:].data_ptr(), L.stream_ptr()))
+        # carry the last 7 windows for the next batch (ball_tracker.py:523), which may start another clip
         carry = eng.pred[nb:nb + 7].clone()
         eng.pred[:7].copy_(carry)
-        self.n_windows += nb
+        host = self._host_ring[slot]
+        host[:nframes].copy_(self.bbox[:nframes], non_blocking=True)
         done = torch.cuda.Event()
         done.record()
-
         state = {"result": None}
 
         def finish():
             if state["result"] is None:
                 done.synchronize()
-                state["result"] = (w0, host[:nframes].numpy().copy())
+                state["result"] = (key, host[:nframes].numpy().copy())
                 self._pending[slot] = None
             return state["result"]
 
         self._pending[slot] = finish
+        # the caller may enqueue more batches before collecting this one: the next slot's launch (three launches back),
+        # if still uncollected, is waited for now, after this batch is enqueued, so the next launch can reuse its slot
+        if self._pending[self._turn] is not None:
+            self._pending[self._turn]()
         return finish
 
 
 class ClipBallPipeline(BallPipeline):
     """BallPipeline over a list of clips in one stream: a device batch may hold the windows of several clips.  The
     host plan (`clip_plan.plan_clip_batches`) says where each frame goes in the ring, when each clip's background is
-    loaded into the median pool and which windows every batch runs; the device gathers each row from its own ring slot
-    and median (`pb_tracknet_pack_windows_rows`) and ensembles each emitted frame over its own clip's windows only
-    (`pb_tracknet_ensemble_rows`).  Per clip the boxes are bit-identical to BallPipeline run on that clip alone."""
+    loaded into the median pool and which windows every batch runs; each row of a batch gathers from its own ring slot
+    and median, and each emitted frame is ensembled over its own clip's windows only.  Per clip the boxes are
+    bit-identical to BallPipeline run on that clip alone."""
 
     def __init__(self, engine: TrackNetEngine, frame_hw: tuple[int, int], ring: int | None = None,
                  pool: int | None = None):
         from .clip_plan import default_pool, default_ring
 
-        self._init_resize(engine, frame_hw)
-        B, H, W = self.B, engine.H, engine.W
-        self.ring = default_ring(B) if ring is None else ring
-        self.pool = default_pool(self.ring) if pool is None else pool
-        self.max_frames = 8 * B  # a window emits its own frame, plus the 7 tail frames when it ends its clip
-        self.small = torch.zeros((self.ring, H, W, 4), dtype=torch.float16, device=self.dev)
-        self.medians = torch.zeros((self.pool, H, W, 4), dtype=torch.float16, device=self.dev)
-        self.tmp = torch.zeros((B + 7, self.Hs, W, 3), dtype=torch.uint8, device=self.dev)
-        self.mask = torch.zeros((self.max_frames, H, W), dtype=torch.uint8, device=self.dev)
-        self.scratch = torch.zeros((B + 7, 5, H * W), dtype=torch.int32, device=self.dev)  # boxes run B+7 at a time
-        self.bbox = torch.zeros((self.max_frames, 4), dtype=torch.int32, device=self.dev)
-        self._host_ring = [torch.zeros((self.max_frames, 4), dtype=torch.int32).pin_memory() for _ in range(3)]
-        self._pending = [None] * 3
-        self._turn = 0
-        self.plan = None
+        ring = default_ring(engine.B) if ring is None else ring
+        # a window emits its own frame, plus the 7 tail frames when it ends its clip
+        self._init_buffers(engine, frame_hw, ring, default_pool(ring) if pool is None else pool, 8 * engine.B)
 
     def begin(self, plan) -> None:
-        """Upload every batch's row and frame tables of `plan` (a ClipPlan with this ring and pool) at once."""
+        """Start the stream of `plan` (a ClipPlan with this ring and pool)."""
         if plan.ring != self.ring or plan.pool != self.pool or plan.batch > self.B or plan.chunk > self.B:
             raise L.PbError("ClipBallPipeline: the plan was made for another ring, pool or batch size")
-        rows, desc, self._tables = [], [], []
-        for ops in plan.steps:
-            for op in ops:
-                if op[0] == "run":
-                    b = op[1]
-                    self._tables.append((len(rows), len(desc)))
-                    rows += list(zip(b.row_slot, b.row_median))
-                    desc += b.desc
-        rows_t = torch.tensor(rows or [(0, 0)], dtype=torch.int32).t().contiguous()
-        self._rows = rows_t.to(self.dev)  # (2, windows): ring slot, median slot
-        self._desc = torch.tensor(desc or [(0, 0, 0)], dtype=torch.int32).to(self.dev)
-        self._next_run = 0
-        self.plan = plan
         self.eng.pred.zero_()
 
     def load_median(self, slot: int, median_rgb: torch.Tensor) -> None:
@@ -369,44 +399,7 @@ class ClipBallPipeline(BallPipeline):
     def run_batch_async(self, batch):
         """Enqueue one planned batch; returns a callable that waits and yields (frames [(clip, frame)], host int32
         (nframes, 4) boxes)."""
-        eng = self.eng
-        nb, nframes = len(batch.windows), len(batch.frames)
-        r0, d0 = self._tables[self._next_run]
-        self._next_run += 1
-        rows = self._rows[:, r0:r0 + nb]
-        L.check(L.lib().pb_tracknet_pack_windows_rows(self.small.data_ptr(), self.ring, rows[0].data_ptr(),
-                                                      self.medians.data_ptr(), rows[1].data_ptr(), nb, eng.H, eng.W,
-                                                      eng.x.data_ptr(), L.stream_ptr()))
-        eng.run_packed()
-        L.check(L.lib().pb_tracknet_ensemble_rows(eng.pred.data_ptr(), batch.first_window - 7,
-                                                  self._desc[d0:d0 + nframes].data_ptr(), nframes, eng.H, eng.W, 0.5,
-                                                  self.mask.data_ptr(), None, L.stream_ptr()))
-        step = self.scratch.shape[0]
-        for f in range(0, nframes, step):  # the scratch holds B+7 frames: several launches for the short-clip case
-            n = min(step, nframes - f)
-            L.check(L.lib().pb_ccl_bbox(self.mask[f:].data_ptr(), n, eng.H, eng.W, self.scratch.data_ptr(),
-                                        self.bbox[f:].data_ptr(), L.stream_ptr()))
-        slot = self._turn
-        self._turn = (slot + 1) % len(self._host_ring)
-        if self._pending[slot] is not None:
-            self._pending[slot]()
-        host = self._host_ring[slot]
-        host[:nframes].copy_(self.bbox[:nframes], non_blocking=True)
-        carry = eng.pred[nb:nb + 7].clone()  # the last 7 windows, for the next batch (which may start another clip)
-        eng.pred[:7].copy_(carry)
-        done = torch.cuda.Event()
-        done.record()
-        state = {"result": None}
-
-        def finish():
-            if state["result"] is None:
-                done.synchronize()
-                state["result"] = (batch.frames, host[:nframes].numpy().copy())
-                self._pending[slot] = None
-            return state["result"]
-
-        self._pending[slot] = finish
-        return finish
+        return self._launch_batch(batch.frames, batch.first_window, batch.row_slot, batch.row_median, batch.desc)
 
 
 def bbox_to_xyv(bbox: np.ndarray, img_scaler: tuple[float, float]):

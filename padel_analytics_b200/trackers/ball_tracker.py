@@ -13,6 +13,7 @@ Documented deviations from reference quirks (SURVEY App. E):
 """
 from __future__ import annotations
 
+import itertools
 import math
 from pathlib import Path
 from typing import Iterable, Optional, Type
@@ -156,8 +157,6 @@ class BallTracker(Tracker):
                   emit_range: Optional[tuple[int, int]] = None, median: Optional[np.ndarray] = None):
         """TrackNet stage on device.  Frames from the generator are absolute frames first_frame, first_frame+1, ...
         Returns dict frame_index -> (x, y, vis) for the frames emitted (restricted to emit_range if given)."""
-        import itertools
-
         it = iter(frame_generator)
         B = self.batch_size
         pending: list[np.ndarray] = []
@@ -174,24 +173,12 @@ class BallTracker(Tracker):
         first = next(stream, None)
         if first is None:
             return {}
-        pipe = self._pipeline(tuple(first.shape[-3:-1]), median)
-        pipe.reset(base=first_frame)
-        w_scaler, h_scaler = self.video_info.width / self.WIDTH, self.video_info.height / self.HEIGHT  # :379-384
+        self.stream_begin(tuple(first.shape[-3:-1]), total_frames, first_frame, emit_range, median)  # :379-384
         out: dict[int, tuple[int, int, int]] = {}
-        total_windows = total_frames - 7
 
         def push(frames):
-            pipe.push_frames(frames if isinstance(frames, torch.Tensor) else torch.from_numpy(np.stack(frames)))
-            while True:  # run every window that became computable
-                nb = min(B, pipe.windows_ready(), total_windows - (pipe.base + pipe.n_windows))
-                if nb <= 0:
-                    return
-                f0, bbox = pipe.run_windows(nb, total_frames)
-                xs, ys, vs = bbox_to_xyv(bbox, (w_scaler, h_scaler))
-                for i in range(len(xs)):
-                    n = f0 + i
-                    if emit_range is None or emit_range[0] <= n < emit_range[1]:
-                        out[n] = (xs[i], ys[i], vs[i])
+            out.update(self.stream_push_async(frames if isinstance(frames, torch.Tensor) else
+                                              torch.from_numpy(np.stack(frames)))())
 
         if isinstance(first, torch.Tensor) and first.dim() == 4:
             # batched frame source: items are uint8 (n,H,W,3) tensors (pinned host or device), n <= batch_size
@@ -236,6 +223,20 @@ class BallTracker(Tracker):
             self._clip_pipe = ClipBallPipeline(self.tracknet, tuple(frame_hw))
         return self._clip_pipe
 
+    def _xyv_finish(self, fins, frames_of):
+        """A callable that waits for the launches `fins` in turn and returns [(frame, (x, y, vis))] for their boxes;
+        frames_of(key) gives the frames of the launch that yields (key, boxes)."""
+        scaler = self._stream["scaler"]
+
+        def finish():
+            out = []
+            for fin in fins:
+                key, bbox = fin()
+                out += zip(frames_of(key), zip(*bbox_to_xyv(bbox, scaler)))
+            return out
+
+        return finish
+
     def _clips_push_async(self, frames: torch.Tensor):
         pipe, s = self._clip_pipe, self._stream
         ops = s["clips"].steps[s["step"]]
@@ -252,16 +253,8 @@ class BallTracker(Tracker):
                 pipe.push_at(frames[off:off + n], slot)
             else:
                 fins.append(pipe.run_batch_async(op[1]))
-
-        def finish():
-            out = []
-            for fin in fins:
-                frames_cf, bbox = fin()
-                xs, ys, vs = bbox_to_xyv(bbox, s["scaler"])
-                out += [(c, f, (xs[i], ys[i], vs[i])) for i, (c, f) in enumerate(frames_cf)]
-            return out
-
-        return finish
+        fin = self._xyv_finish(fins, lambda frames: frames)  # a batch yields its [(clip, frame)]
+        return lambda: [(c, f, v) for (c, f), v in fin()]
 
     def stream_push_async(self, frames: torch.Tensor):
         """frames: uint8 (n,H,W,3) BGR tensor (device or pinned host), n <= batch_size.  Enqueues resize + every
@@ -270,28 +263,9 @@ class BallTracker(Tracker):
             return self._clips_push_async(frames)
         pipe, s = self._pipe, self._stream
         pipe.push_frames(frames)
-        fins = []
-        while True:
-            nb = min(self.batch_size, pipe.windows_ready(), s["total"] - 7 - (pipe.base + pipe.n_windows))
-            if nb <= 0:
-                break
-            if fins:  # only one launch may be in flight per pipeline: resolve the previous one first
-                res = fins[-1]()
-                fins[-1] = (lambda r: (lambda: r))(res)
-            fins.append(pipe.run_windows_async(nb, s["total"]))
-
-        def finish():
-            out = {}
-            for fin in fins:
-                f0, bbox = fin()
-                xs, ys, vs = bbox_to_xyv(bbox, s["scaler"])
-                for i in range(len(xs)):
-                    n = f0 + i
-                    if s["emit"] is None or s["emit"][0] <= n < s["emit"][1]:
-                        out[n] = (xs[i], ys[i], vs[i])
-            return out
-
-        return finish
+        fin = self._xyv_finish(pipe.run_ready_async(s["total"]), itertools.count)  # a launch yields its first frame
+        emit = s["emit"]
+        return lambda: {n: v for n, v in fin() if emit is None or emit[0] <= n < emit[1]}
 
     # ---- InpaintNet stage (ball_tracker.py:525-673) -------------------------------------------------------------
     @staticmethod

@@ -330,7 +330,7 @@ def test_ccl_rejects_bad_shapes_before_launch():
     torch.cuda.synchronize()
 
 
-# ---- d. pb_tracknet_ensemble in isolation -----------------------------------------------------------------------------
+# ---- d. pb_tracknet_ensemble_rows in isolation ------------------------------------------------------------------------
 @pytest.mark.parametrize("case", ["first", "middle", "tail", "single"])
 def test_ensemble_batch_positions(case):
     H, W, B = R.H_NET, R.W_NET, 8
@@ -348,12 +348,13 @@ def test_ensemble_batch_positions(case):
             buf[s - (w0 - 7)] = preds[s]
     bd = buf.to(DEV)
     nfr = nb + (7 if w0 + nb == S else 0)
+    desc = torch.tensor([(0, S, n) for n in range(w0, w0 + nfr)], dtype=torch.int32, device=DEV)  # the video's clip
     masks, ens = [], None
     for want in (True, False):
         mask = torch.full((nfr, H, W), 7, dtype=torch.uint8, device=DEV)
         e = torch.full((nfr, H, W), -1.0, device=DEV) if want else None
-        L.check(L.lib().pb_tracknet_ensemble(bd.data_ptr(), 7 + nb, w0 - 7, S, w0, nfr, H, W, 0.5, mask.data_ptr(),
-                                             L.ptr(e), L.stream_ptr()))
+        L.check(L.lib().pb_tracknet_ensemble_rows(bd.data_ptr(), w0 - 7, desc.data_ptr(), nfr, H, W, 0.5,
+                                                  mask.data_ptr(), L.ptr(e), L.stream_ptr()))
         torch.cuda.synchronize()
         masks.append(mask.cpu())
         ens = e.cpu() if want else ens
@@ -363,17 +364,20 @@ def test_ensemble_batch_positions(case):
     print(f"ensemble {case}: frames {w0}..{w0 + nfr - 1} of {T}, {int(masks[0].sum())} foreground pixels")
 
 
-def test_ensemble_rejects_missing_windows():
-    H, W = 16, 16
-    buf = torch.zeros((15, 8, H, W), device=DEV)
-    mask = torch.zeros((15, H, W), dtype=torch.uint8, device=DEV)
-    # 33 windows (T = 40); a valid call first, then a buffer missing the first / last needed window
-    L.check(L.lib().pb_tracknet_ensemble(buf.data_ptr(), 15, -7, 33, 0, 8, H, W, 0.5, mask.data_ptr(), None,
-                                         L.stream_ptr()))
+def test_ensemble_rejects_missing_windows(tracknet_ckpt):
+    """A batch whose frames need windows outside the heat-map buffer (the 7 carried windows and the batch's own) is
+    refused on the host, before any device work is enqueued."""
+    pipe = BallPipeline(_engine(tracknet_ckpt, 8, SMALL_HW), SRC_HW, synth.make_median(*SRC_HW).numpy())
+    desc = lambda frame0, nframes: [(0, 33, n) for n in range(frame0, frame0 + nframes)]  # 33 windows (T = 40)
+    # a valid batch first: 8 windows from window 0 emit frames 0..7
+    pipe._launch_batch(0, 0, list(range(8)), [0] * 8, desc(0, 8))()
+    # the same buffers missing the first / last needed window: (buffer rows = 7 + nb, first buffer row's window)
     for S_buf, first_window, frame0, nframes in ((15, 1, 0, 8), (8, 9, 16, 8), (9, 23, 30, 10)):
-        with pytest.raises(L.PbError):
-            L.check(L.lib().pb_tracknet_ensemble(buf.data_ptr(), S_buf, first_window, 33, frame0, nframes, H, W, 0.5,
-                                                 mask.data_ptr(), None, L.stream_ptr()))
+        nb = S_buf - 7
+        launches = L.lib().pb_launch_count()
+        with pytest.raises(L.PbError, match="needs windows"):
+            pipe._launch_batch(0, first_window + 7, list(range(nb)), [0] * nb, desc(frame0, nframes))
+        assert L.lib().pb_launch_count() == launches
     torch.cuda.synchronize()
 
 

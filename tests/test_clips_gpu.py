@@ -1,5 +1,5 @@
-"""Tracking a list of clips in one pass: the two multi-clip kernels against the single-clip kernels, and
-`TrackingRunner.run_clips` against a fresh `TrackingRunner.run()` on each clip alone."""
+"""Tracking a list of clips in one pass: the two multi-clip kernels against a numpy gather and the reference ensemble
+loop per clip, and `TrackingRunner.run_clips` against a fresh `TrackingRunner.run()` on each clip alone."""
 import json
 
 import numpy as np
@@ -7,6 +7,7 @@ import pytest
 import torch
 
 from oracle import inpaint as OI
+from oracle import tracknet as OT
 from oracle import weights as OW
 from padel_analytics_b200 import _lib as L
 from padel_analytics_b200 import synth
@@ -20,69 +21,72 @@ H, W = 1080, 1920
 
 
 def test_pack_windows_rows_equals_per_row_pack():
+    """Every row of one launch over random ring slots and pool medians == the numpy gather of its median and its 8
+    ring slots, bit for bit."""
     Hn, Wn, ring, pool, B = 24, 40, 29, 5, 13
     g = torch.Generator().manual_seed(3)
-    frames = torch.randint(0, 1 << 15, (ring, Hn, Wn, 4), generator=g, dtype=torch.int16).cuda()
-    meds = torch.randint(0, 1 << 15, (pool, Hn, Wn, 4), generator=g, dtype=torch.int16).cuda()
+    frames = torch.randint(0, 1 << 15, (ring, Hn, Wn, 4), generator=g, dtype=torch.int16)
+    meds = torch.randint(0, 1 << 15, (pool, Hn, Wn, 4), generator=g, dtype=torch.int16)
     slots = torch.randint(0, ring, (B,), generator=g, dtype=torch.int32)
     slots[3] = ring - 1  # a window that wraps the ring
     mids = torch.randint(0, pool, (B,), generator=g, dtype=torch.int32)
     x = torch.full((B, Hn, Wn, 32), 7, dtype=torch.int16, device="cuda")
-    slots_d, mids_d = slots.cuda(), mids.cuda()
-    L.check(L.lib().pb_tracknet_pack_windows_rows(frames.data_ptr(), ring, slots_d.data_ptr(), meds.data_ptr(),
+    fd, md, slots_d, mids_d = frames.cuda(), meds.cuda(), slots.cuda(), mids.cuda()
+    L.check(L.lib().pb_tracknet_pack_windows_rows(fd.data_ptr(), ring, slots_d.data_ptr(), md.data_ptr(),
                                                   mids_d.data_ptr(), B, Hn, Wn, x.data_ptr(), L.stream_ptr()))
-    one = torch.full((1, Hn, Wn, 32), 9, dtype=torch.int16, device="cuda")
+    got = x.cpu().numpy()
+    fr, me = frames.numpy(), meds.numpy()
     for b in range(B):
-        L.check(L.lib().pb_tracknet_pack_windows(frames.data_ptr(), ring, int(slots[b]), meds[int(mids[b])].data_ptr(),
-                                                 1, Hn, Wn, one.data_ptr(), L.stream_ptr()))
-        assert torch.equal(x[b], one[0]), b
+        chans = [me[mids[b], ..., :3]] + [fr[(int(slots[b]) + f) % ring, ..., :3] for f in range(8)]
+        exp = np.concatenate(chans + [np.zeros((Hn, Wn, 5), np.int16)], -1)
+        assert np.array_equal(got[b], exp), b
 
 
 @pytest.mark.parametrize("lengths,batch", [([5, 8, 9, 40, 77, 130], 32), ([8, 9, 8, 15, 3, 23, 8], 4),
                                            ([20, 8, 8, 8, 12], 16), ([30, 2, 30], 1)])
 def test_ensemble_rows_equals_per_clip_ensemble(lengths, batch):
-    """Every planned batch: one pb_tracknet_ensemble_rows launch == pb_tracknet_ensemble called on each clip's frames
-    of the batch (mask and ensemble, bit for bit), with the engine's pred ring and 7-row carry."""
+    """Every planned batch through pb_tracknet_ensemble_rows, with the engine's pred ring and 7-row carry: each clip's
+    frames == oracle/tracknet.py's stateful ensemble loop run on that clip alone (ensemble bit for bit, and the mask
+    is its threshold)."""
     Hn, Wn = 288, 512
     g = torch.Generator().manual_seed(len(lengths) * 100 + batch)
     plan = plan_clip_batches(lengths, batch)
-    nw = sum(max(0, t - 7) for t in lengths)
-    heat = torch.rand((nw, 8, Hn, Wn), generator=g)
+    nw = [max(0, t - 7) for t in lengths]
+    heat = torch.rand((sum(nw), 8, Hn, Wn), generator=g)
     heat.view(-1)[::5] = 0.5  # many ensembled pixels land on the threshold
-    heat = heat.cuda()
+    heat_d = heat.cuda()
     pred = torch.zeros((7 + batch, 8, Hn, Wn), device="cuda")
     maxf = 8 * batch
     mask, ens = (torch.empty((maxf, Hn, Wn), dtype=torch.uint8, device="cuda"),
                  torch.empty((maxf, Hn, Wn), device="cuda"))
-    mask1, ens1 = torch.empty_like(mask), torch.empty_like(ens)
-    spans = 0
+    got, spans = {}, 0
     for ops in plan.steps:
         for op in ops:
             if op[0] != "run":
                 continue
             b = op[1]
             nb, nf = len(b.windows), len(b.frames)
-            pred[7:7 + nb] = heat[b.first_window:b.first_window + nb]
+            pred[7:7 + nb] = heat_d[b.first_window:b.first_window + nb]
             desc = torch.tensor(b.desc, dtype=torch.int32).cuda()
             L.check(L.lib().pb_tracknet_ensemble_rows(pred.data_ptr(), b.first_window - 7, desc.data_ptr(), nf, Hn, Wn,
                                                       0.5, mask.data_ptr(), ens.data_ptr(), L.stream_ptr()))
-            i = 0
-            clips = 0
-            while i < nf:  # each clip's run of frames through the single-clip kernel
-                c = b.frames[i][0]
-                j = i
-                while j < nf and b.frames[j][0] == c:
-                    j += 1
-                cw0, tw, f0 = b.desc[i]
-                L.check(L.lib().pb_tracknet_ensemble(pred.data_ptr(), 7 + nb, b.first_window - 7 - cw0, tw, f0, j - i,
-                                                     Hn, Wn, 0.5, mask1[i:].data_ptr(), ens1[i:].data_ptr(),
-                                                     L.stream_ptr()))
-                i, clips = j, clips + 1
-            spans += clips > 1
-            assert torch.equal(mask[:nf], mask1[:nf]) and torch.equal(ens[:nf], ens1[:nf]), b.first_window
+            m, e = mask[:nf].cpu(), ens[:nf].cpu()
+            for i, cf in enumerate(b.frames):
+                got[cf] = (m[i], e[i])
+            spans += len({c for c, _ in b.frames}) > 1
             pred[:7] = pred[nb:nb + 7].clone()
     if batch > 1:  # a one-window batch emits one clip's frames only
         assert spans, "vacuous: no batch emitted frames of two clips"
+    w0 = 0
+    for c, t in enumerate(lengths):
+        exp = OT.ensemble_reference_loop(heat[w0:w0 + nw[c]], t, batch)
+        w0 += nw[c]
+        assert len(exp) == (t if t >= 8 else 0)
+        for f in range(len(exp)):
+            m, e = got.pop((c, f))
+            assert torch.equal(e, exp[f]), (c, f)
+            assert torch.equal(m.bool(), exp[f] > 0.5), (c, f)
+    assert not got
 
 
 # ---- end to end ------------------------------------------------------------------------------------------------------

@@ -50,7 +50,7 @@ def test_ball_pipeline_matches_oracle():
     for i in range(B):
         ref = OT.resize_rgb(fr_np[i][..., ::-1].copy())
         assert torch.equal(small[i], to16(ref))
-    assert torch.equal(pipe.median_small[0, ..., :3].cpu(), to16(OT.resize_rgb(med.numpy())))
+    assert torch.equal(pipe.medians[0, ..., :3].cpu(), to16(OT.resize_rgb(med.numpy())))
     got = {}
     ens_all = {}
     pushed = B

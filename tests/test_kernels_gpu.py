@@ -84,18 +84,19 @@ def test_tracknet_pack_windows():
     rng = np.random.default_rng(2)
     ring, B, H, W = 12, 4, 32, 64
     frames = rng.integers(0, 256, (ring, H, W, 3), dtype=np.uint8)
-    med = rng.integers(0, 256, (H, W, 3), dtype=np.uint8)
+    meds = rng.integers(0, 256, (2, H, W, 3), dtype=np.uint8)
     to4 = lambda a: torch.cat([(torch.from_numpy(a).float() * np.float32(1 / 255.0)).half(),
                                torch.zeros(a.shape[:-1] + (1,), dtype=torch.float16)], -1).contiguous().to(DEV)
     x = torch.zeros((B, H, W, 32), dtype=torch.float16, device=DEV)
-    first = 7
-    fd, md = to4(frames), to4(med)
-    L.check(L.lib().pb_tracknet_pack_windows(fd.data_ptr(), ring, first, md.data_ptr(), B, H, W, x.data_ptr(),
-                                             L.stream_ptr()))
+    slots, mids = [7, 11, 0, 5], [0, 1, 1, 0]  # rows 0 and 1 wrap the ring
+    fd, md = to4(frames), to4(meds)
+    sd, mdd = (torch.tensor(v, dtype=torch.int32, device=DEV) for v in (slots, mids))
+    L.check(L.lib().pb_tracknet_pack_windows_rows(fd.data_ptr(), ring, sd.data_ptr(), md.data_ptr(), mdd.data_ptr(),
+                                                  B, H, W, x.data_ptr(), L.stream_ptr()))
     torch.cuda.synchronize()
     got = x.cpu().float()
     for b in range(B):
-        chans = [med] + [frames[(first + b + f) % ring] for f in range(8)]
+        chans = [meds[mids[b]]] + [frames[(slots[b] + f) % ring] for f in range(8)]
         exp = np.concatenate(chans, -1).astype(np.float64) / 255.0  # iterable.py:186-197
         assert np.abs(got[b, ..., :27].numpy() - exp).max() < 6e-4
         assert torch.all(got[b, ..., 27:] == 0)
@@ -115,10 +116,11 @@ def test_ensemble_matches_reference_loop(T, bs):
         nb = min(bs, S - w0)
         buf[7:7 + nb] = preds[w0:w0 + nb].to(DEV)
         nfr = nb + (7 if w0 + nb == S else 0)
+        desc = torch.tensor([(0, S, n) for n in range(w0, w0 + nfr)], dtype=torch.int32, device=DEV)  # one clip
         mask = torch.zeros((nfr, H, W), dtype=torch.uint8, device=DEV)
         ens = torch.zeros((nfr, H, W), device=DEV)
-        L.check(L.lib().pb_tracknet_ensemble(buf.data_ptr(), 7 + nb, w0 - 7, S, w0, nfr, H, W, 0.5, mask.data_ptr(),
-                                             ens.data_ptr(), L.stream_ptr()))
+        L.check(L.lib().pb_tracknet_ensemble_rows(buf.data_ptr(), w0 - 7, desc.data_ptr(), nfr, H, W, 0.5,
+                                                  mask.data_ptr(), ens.data_ptr(), L.stream_ptr()))
         torch.cuda.synchronize()
         got.append(ens.cpu())
         assert torch.equal(mask.cpu().bool(), ens.cpu() > 0.5)
