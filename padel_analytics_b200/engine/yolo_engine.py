@@ -533,7 +533,6 @@ class YoloEngine:
             out += self._results(rows, counts, len(chunk), (st["Hn"], st["Wn"]), orig)
         return out
 
-    @torch.no_grad()
     def predict_frames(self, frames, prep: str, conf, iou, imgsz, classes=None, max_det=300):
         """Fused fast path used by this repo's trackers: raw BGR video frames in, all pre-processing on device.
         prep='letterbox_q1': PlayerTracker path (processor BGR->RGB + ultralytics' own flip => the network sees the
@@ -541,16 +540,7 @@ class YoloEngine:
         prep='pil_square' : PlayerKeypoints/Keypoints path (BGR->RGB, PIL resize to imgsz x imgsz).
         Returned coordinates are in the pre-processed image's pixel space, exactly like model.predict() on the
         processed sample (full frame for letterbox_q1, imgsz x imgsz for pil_square)."""
-        fr = self._upload(frames)
-        n = fr.shape[0]
-        if prep == "letterbox_q1":
-            st, orig = self._letterbox(fr, imgsz, (0, 1, 2))
-        elif prep == "pil_square":
-            st, orig = self._pil_square(fr, imgsz)
-        else:
-            raise L.PbError(f"unknown prep {prep!r}")
-        rows, counts = self._detect(st, n, conf, iou, classes, max_det)
-        return self._results_block(rows, counts, n, (st["Hn"], st["Wn"]), orig)
+        return self.predict_frames_async(frames, prep, conf, iou, imgsz, classes, max_det)()
 
     @torch.no_grad()
     def predict_frames_async(self, frames, prep: str, conf, iou, imgsz, classes=None, max_det=300):

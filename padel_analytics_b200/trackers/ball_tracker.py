@@ -88,6 +88,7 @@ def median_background_device(frames_bgr, device="cuda") -> torch.Tensor:
 
 
 class BallTracker(Tracker):
+    stage = "ball"
     EVAL_MODE: str = "weight"
     TRAJECTORY_LENGTH: int = 8
     HEIGHT: int = 288
@@ -358,13 +359,12 @@ class BallTracker(Tracker):
         out.update({lo + k: v for k, v in res.items()})
         return out
 
+    def balls(self, xyv: dict, total_frames: int) -> list[Ball]:
+        """A video's or clip's TrackNet trajectory {frame: (x, y, vis)} -> the InpaintNet stage (`inpaint_xyv`) -> one
+        Ball per frame 0..total_frames-1 (ball_tracker.py:675-698: missing frames -> (0,0), visibility 0)."""
+        xyv = self.inpaint_xyv(xyv, total_frames)
+        return [Ball(frame=n, xy=(xyv[n][0], xyv[n][1]), visibility=xyv[n][2]) if n in xyv
+                else Ball(frame=n, xy=(0.0, 0.0), visibility=0) for n in range(total_frames)]
+
     def predict_frames(self, frame_generator: Iterable[np.ndarray], total_frames: int, **kwargs) -> list[Ball]:
-        xyv = self.inpaint_xyv(self.track_xyv(frame_generator, total_frames), total_frames)
-        balls = []
-        for n in range(total_frames):  # ball_tracker.py:675-698 (missing frames -> (0,0), visibility 0)
-            if n in xyv:
-                x, y, v = xyv[n]
-                balls.append(Ball(frame=n, xy=(x, y), visibility=v))
-            else:
-                balls.append(Ball(frame=n, xy=(0.0, 0.0), visibility=0))
-        return balls
+        return self.balls(self.track_xyv(frame_generator, total_frames), total_frames)

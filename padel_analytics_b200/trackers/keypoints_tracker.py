@@ -112,9 +112,17 @@ class KeypointsTracker(Tracker):
         if self.model is not None:
             self.model.to(device)
 
-    def detect_sample(self, sample):
-        return self.model.predict_frames(sample, "pil_square", conf=self.CONF, iou=self.IOU,
-                                         imgsz=self.TRAIN_IMAGE_SIZE, classes=None, max_det=self.NUMBER_KEYPOINTS)
+    @property
+    def stage(self) -> str:
+        """The runner stage: "fixed" with a fixed detection, "detect" for a YOLO model, else "frames" (the ResNet
+        regressor runs through predict_frames, as the reference's does)."""
+        if self.fixed_keypoints_detection is not None:
+            return "fixed"
+        return "detect" if self.model_type == "yolo" and self.model is not None else "frames"
+
+    @property
+    def fixed_detection(self) -> Optional[Keypoints]:
+        return self.fixed_keypoints_detection
 
     def detect_sample_async(self, sample):
         return self.model.predict_frames_async(sample, "pil_square", conf=self.CONF, iou=self.IOU,

@@ -141,6 +141,7 @@ class PlayersKeypoints(Object):
 
 
 class PlayerKeypointsTracker(Tracker):
+    stage = "detect"
     CONF = 0.25
     IOU = 0.7
 
@@ -169,10 +170,6 @@ class PlayerKeypointsTracker(Tracker):
 
     def to(self, device: str) -> None:
         self.model.to(device)
-
-    def detect_sample(self, sample):
-        return self.model.predict_frames(sample, "pil_square", conf=self.CONF, iou=self.IOU,
-                                         imgsz=self.train_image_size, classes=[0])
 
     def detect_sample_async(self, sample):
         return self.model.predict_frames_async(sample, "pil_square", conf=self.CONF, iou=self.IOU,

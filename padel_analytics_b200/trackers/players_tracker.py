@@ -147,6 +147,7 @@ class Players(Object):
 
 
 class PlayerTracker(Tracker):
+    stage = "detect"
     CONF = 0.5
     IOU = 0.7
     IMGSZ = 640
@@ -182,18 +183,15 @@ class PlayerTracker(Tracker):
     def to(self, device: str) -> None:
         self.model.to(device)
 
-    def detect_sample(self, sample):
-        """Model stage only (boxes in frame pixels), shard-safe: no sequential state."""
-        return self.model.predict_frames(sample, "letterbox_q1", conf=self.CONF, iou=self.IOU, imgsz=self.IMGSZ,
-                                         classes=[0])
-
     def detect_sample_async(self, sample):
-        """Enqueue the model stage; returns a callable yielding the raw results (see YoloEngine.predict_frames_async)."""
+        """Enqueue the model stage (boxes in frame pixels); returns a callable yielding the raw results (see
+        YoloEngine.predict_frames_async)."""
         return self.model.predict_frames_async(sample, "letterbox_q1", conf=self.CONF, iou=self.IOU,
                                                imgsz=self.IMGSZ, classes=[0])
 
-    def postprocess(self, results) -> list[Players]:
-        """Polygon filter + ByteTrack ids (players_tracker.py:362-378); sequential, frame order matters."""
+    def postprocess(self, results, frame_hw=None) -> list[Players]:
+        """Polygon filter + ByteTrack ids (players_tracker.py:362-378); sequential, frame order matters.  The boxes
+        are already in frame pixels, so `frame_hw` is not needed."""
         if isinstance(results, ResultBlock) and hasattr(self.byte_track, "update_many"):
             return self._postprocess_block(results)
         out = []

@@ -31,9 +31,8 @@ from . import frames
 from . import sv_compat as sv
 from ..engine.yolo_engine import ResultBlock
 from .ball_tracker import Ball, BallTracker
-from .keypoints_tracker import Keypoints, KeypointsTracker
-from .players_keypoints_tracker import PlayerKeypointsTracker
-from .players_tracker import PlayerTracker, Players
+from .keypoints_tracker import Keypoints
+from .players_tracker import Players
 from .tracker import Tracker, sampler
 from ..analytics import DataAnalytics, ProjectedCourt
 
@@ -69,6 +68,11 @@ def ball_shard_frames(total: int, start: int, end: int) -> tuple[int, int]:
     return max(0, start - 7), min(total, end + 7)
 
 
+def _batch_trackers(trackers: dict[str, Tracker]) -> dict[str, Tracker]:
+    """The trackers a device pass (`FusedPass`, `ClipPass`) feeds: those of stage "detect" or "ball"."""
+    return {n: t for n, t in trackers.items() if t.stage in ("detect", "ball")}
+
+
 class FusedPass:
     """One pass over the video feeding ALL trackers from a single upload per batch (the reference decodes and uploads
     the video once per tracker, runner.py:185-234; SURVEY §8f item 3).  Per batch: the next batch's host->device copy
@@ -92,7 +96,7 @@ class FusedPass:
         self.mode = int(os.environ.get("PADEL_B200_STREAMS", "1")) if streams is None else streams
         # side streams: the YOLO chains at high priority (their CTAs are placed first whenever SMs free up), the ball
         # tracker (mode 2 only) at normal priority
-        self.side = {name: torch.cuda.Stream(priority=0 if isinstance(t, BallTracker) else -1)
+        self.side = {name: torch.cuda.Stream(priority=0 if t.stage == "ball" else -1)
                      for name, t in trackers.items()}
         self.hw = tuple(frame_hw)
         self.B = batch_size
@@ -106,7 +110,7 @@ class FusedPass:
 
     def _begin_ball(self, total_frames, first_frame, emit_range, median) -> None:
         for t in self.trackers.values():
-            if isinstance(t, BallTracker):
+            if t.stage == "ball":
                 t.stream_begin(self.hw, total_frames, first_frame, emit_range, median=median)
 
     def _upload(self, pieces, slot: int) -> torch.Tensor:
@@ -140,12 +144,9 @@ class FusedPass:
         forked = []
         order = list(self.trackers.items())
         if self.mode == 1:  # YOLO chains first (concurrent), the ball tracker joins behind them
-            order.sort(key=lambda kv: isinstance(kv[1], BallTracker))
+            order.sort(key=lambda kv: kv[1].stage == "ball")
         for name, t in order:  # enqueue everything first ...
-            if getattr(t, "fixed_keypoints_detection", None) is not None:
-                pending.append((name, t, None))
-                continue
-            is_ball = isinstance(t, BallTracker)
+            is_ball = t.stage == "ball"
             own = self.mode == 2 or (self.mode == 1 and not is_ball)
             if own:
                 s = self.side[name]
@@ -166,19 +167,11 @@ class FusedPass:
 
     def _finish(self, launched) -> dict:
         """Wait for each tracker's results in turn and run its host post-processing."""
-        pending, nfr = launched
+        pending, _ = launched
         out = {}
         for name, t, fin in pending:  # ... then finish in the same order
-            if isinstance(t, BallTracker):
-                out[name] = fin()
-            elif fin is None:
-                out[name] = [t.fixed_keypoints_detection] * nfr
-            elif self.raw:
-                out[name] = fin()
-            elif isinstance(t, PlayerTracker):
-                out[name] = t.postprocess(fin())
-            else:
-                out[name] = t.postprocess(fin(), self.hw)
+            res = fin()
+            out[name] = res if t.stage == "ball" or self.raw else t.postprocess(res, self.hw)
         return out
 
     def run(self, batches: Iterable):
@@ -239,7 +232,7 @@ class ClipPass(FusedPass):
         from ..engine.clip_plan import plan_clip_batches
 
         for t in self.trackers.values():
-            if isinstance(t, BallTracker):
+            if t.stage == "ball":
                 pipe = t.clip_pipeline(self.hw)
                 plan = plan_clip_batches(self.lengths, t.batch_size, chunk=self.B, ring=pipe.ring, pool=pipe.pool)
                 t.clips_begin(self.hw, plan, self.median_of)
@@ -255,15 +248,14 @@ class ClipPass(FusedPass):
         self._pos = base + nfr
         out = {}
         for name, t, fin in pending:
-            if isinstance(t, BallTracker):
+            if t.stage == "ball":
                 out[name] = fin()
                 continue
             res, parts = fin(), []
             for c, a, b, f0 in segs:
                 if f0 == 0:
                     t.video_info_post_init(self.clip_infos[c])
-                piece = res[a:b]
-                parts.append((c, t.postprocess(piece) if isinstance(t, PlayerTracker) else t.postprocess(piece, self.hw)))
+                parts.append((c, t.postprocess(res[a:b], self.hw)))
             out[name] = parts
         return out
 
@@ -287,8 +279,7 @@ class TrackingRunner:
             for t in self.trackers.values():
                 t.video_info_post_init(video_info)  # runner.py:61-62
         # runner.py:59-79: fixed court keypoints keep the first homography; the mini court needs the frame size
-        self.is_fixed_keypoints = any(getattr(t, "fixed_keypoints_detection", None) is not None
-                                      for t in self.trackers.values() if isinstance(t, KeypointsTracker))
+        self.is_fixed_keypoints = any(t.stage == "fixed" for t in self.trackers.values())
         self.collect_data = collect_data
         self.projected_court = ProjectedCourt(video_info) if video_info is not None else None
         self.data_analytics = DataAnalytics() if collect_data else None
@@ -312,10 +303,11 @@ class TrackingRunner:
         """The runner pass (runner.py:185-234).  `frame_source(lo, hi)` yields frames lo..hi-1 (defaults to decoding
         `video_path`).
 
-        fused (default: on when two or more trackers still need inference): ONE pass over the frames feeds every
-        such tracker from a single decode + upload per batch (`FusedPass`; the reference decodes and uploads once per
-        tracker, runner.py:215-220).  fused=False is the reference's plain loop, one full pass per tracker.
-        Trackers with cached predictions (runner.py:187-191) or a fixed keypoints detection never enter the fused set.
+        fused (default: on when two or more trackers of stage "detect" or "ball" still need inference): ONE pass over
+        the frames feeds every such tracker from a single decode + upload per batch (`FusedPass`; the reference decodes
+        and uploads once per tracker, runner.py:215-220).  fused=False is the reference's plain loop, one full pass per
+        tracker.  Trackers with cached predictions (runner.py:187-191) are skipped; those of stage "fixed" or "frames"
+        run through `predict_and_update`.
 
         Under torch.distributed (world_size > 1) each rank processes its contiguous shard, fixed-capacity detection
         records are all-gathered, and rank 0 runs the order-dependent host stages (polygon filter, ByteTrack ids,
@@ -351,8 +343,7 @@ class TrackingRunner:
         rank, world = (dist.get_rank(), dist.get_world_size()) if dist_on else (0, 1)
         lo, hi = shard_range(total, rank, world)
         todo = {n: t for n, t in self.trackers.items() if len(t) == 0}  # cached predictions: skipped (runner.py:187-191)
-        model = {n: t for n, t in todo.items() if isinstance(t, (PlayerTracker, PlayerKeypointsTracker, BallTracker))
-                 or (isinstance(t, KeypointsTracker) and t.fixed_keypoints_detection is None and t.model is not None)}
+        model = _batch_trackers(todo)
         if fused is None:
             fused = len(model) >= 2 and torch.cuda.is_available()
         if fused and model:
@@ -361,19 +352,18 @@ class TrackingRunner:
         for name, tracker in todo.items():
             tracker.to(tracker.DEVICE)
             t0 = timeit.default_timer()
-            if isinstance(tracker, BallTracker):
+            if tracker.stage == "ball":
                 flo, fhi = ball_shard_frames(total, lo, hi)
                 median = self._ball_median(tracker, src, total, rank, dist_on)
                 part = tracker.track_xyv(src(flo, fhi), total, first_frame=flo, emit_range=(lo, hi), median=median)
                 part = _ball_records(part, lo, hi)
-            elif isinstance(tracker, (PlayerTracker, PlayerKeypointsTracker, KeypointsTracker)) and \
-                    getattr(tracker, "fixed_keypoints_detection", None) is None:
+            elif tracker.stage == "detect":
                 part, hw = [], None
                 for sample in sampler(src(lo, hi), tracker.batch_size):
                     hw = sample[0].shape[:2]
-                    part += tracker.detect_sample(sample)
+                    part.append(tracker.detect_sample(sample))
                 part = (_yolo_records(part, tracker), hw)
-            else:
+            else:  # "frames", and "fixed", whose predict_frames repeats the detection once per frame of the source
                 part = list(tracker.predict_and_update(src(lo, hi), total_frames=hi - lo).predictions)
             if torch.cuda.is_available():
                 torch.cuda.synchronize()
@@ -542,7 +532,7 @@ class TrackingRunner:
     def _run_fused(self, model: dict, src, total: int, lo: int, hi: int, rank: int, world: int, dist_on: bool):
         """One pass over this rank's frames for every tracker in `model`.  A ball shard needs 7 frames of history and
         7 of look-ahead (`ball_shard_frames`); the YOLO results of those halo frames are simply dropped."""
-        ball = next((t for t in model.values() if isinstance(t, BallTracker)), None)
+        ball = next((t for t in model.values() if t.stage == "ball"), None)
         flo, fhi = ball_shard_frames(total, lo, hi) if ball is not None else (lo, hi)
         B = min(t.batch_size for t in model.values())  # every engine is sized for its own tracker's batch_size
         for t in model.values():
@@ -561,30 +551,27 @@ class TrackingRunner:
             pos = flo
             for out in fp.run(itertools.chain([first], chunks)):
                 for name, t in model.items():
-                    if isinstance(t, BallTracker):
-                        parts[name].append(out[name])
-                    else:
-                        res = out[name]
+                    res = out[name]
+                    if t.stage == "ball":
+                        parts[name].append(res)
+                    else:  # ResultBlocks under torch.distributed (raw), else post-processed objects
                         a, b = max(lo - pos, 0), min(hi - pos, len(res))  # halo frames of a ball shard are dropped
                         if b > a:
-                            if isinstance(res, ResultBlock):
-                                parts[name].append(res[a:b])
-                            else:
-                                parts[name] += res[a:b]
+                            parts[name].append(res[a:b])
                 pos += B  # every chunk but the last holds B frames
         torch.cuda.synchronize()
         t_pass = timeit.default_timer() - t0
         t1 = timeit.default_timer()
         for name, t in model.items():
-            if isinstance(t, BallTracker):
+            if t.stage == "ball":
                 xyv = {}
                 for d in parts[name]:
                     xyv.update(d)
                 part = _ball_records(xyv, lo, hi)
-            elif not dist_on or not all(isinstance(p, ResultBlock) for p in parts[name]):
-                part = parts[name]  # already post-processed (or fixed) objects, in frame order
-            else:
+            elif dist_on:
                 part = (_yolo_records(parts[name], t), hw)
+            else:
+                part = [o for p in parts[name] for o in p]  # already post-processed objects, in frame order
             self._gather_and_assemble(t, part, total, rank, world, dist_on)
             self.timings[name] = t_pass  # one shared pass: per-tracker times are not separable
             t.to("cpu")
@@ -613,26 +600,15 @@ class TrackingRunner:
 
     @staticmethod
     def _assemble(tracker: Tracker, parts: list, total: int) -> None:
-        if isinstance(tracker, BallTracker):
+        if tracker.stage == "ball":
             xyv = {}
             for p in parts:
                 xyv.update(p.to_dict() if isinstance(p, BallRecords) else p)
-            xyv = tracker.inpaint_xyv(xyv, total)  # whole-trajectory stage: after the shards are merged
-            tracker.results.predictions = [
-                Ball(frame=n, xy=(xyv[n][0], xyv[n][1]), visibility=xyv[n][2]) if n in xyv
-                else Ball(frame=n, xy=(0.0, 0.0), visibility=0) for n in range(total)]
-        elif parts and isinstance(parts[0], tuple):
+            tracker.results.predictions = tracker.balls(xyv, total)  # InpaintNet: after the shards are merged
+        elif parts and isinstance(parts[0], tuple):  # (YoloRecords, frame size) per shard
             hw = next((h for _, h in parts if h), None)
-            if all(isinstance(res, YoloRecords) for res, _ in parts):  # dense records: stay dense
-                results = ResultBlock.concat([res.to_results(tracker) for res, _ in parts])
-            else:
-                results = []
-                for res, _ in parts:
-                    results += list(res.to_results(tracker)) if isinstance(res, YoloRecords) else list(res)
-            if isinstance(tracker, PlayerTracker):
-                tracker.results.predictions = tracker.postprocess(results)  # ordered => ByteTrack ids are consistent
-            else:
-                tracker.results.predictions = tracker.postprocess(results, hw)
+            results = ResultBlock.concat([res.to_results(tracker) for res, _ in parts])
+            tracker.results.predictions = tracker.postprocess(results, hw)  # ordered => ByteTrack ids are consistent
         else:
             tracker.results.predictions = [o for p in parts for o in p]
 
@@ -735,8 +711,7 @@ class TrackingRunner:
         t0 = timeit.default_timer()
         seen = exchange_clip_status(failure, seen, next((c for c in mine if lengths[c]), None), cause)
         hw = hw if seen is None else seen
-        fixed = {n: t.fixed_keypoints_detection for n, t in self.trackers.items()
-                 if getattr(t, "fixed_keypoints_detection", None) is not None}
+        fixed = {n: t.fixed_detection for n, t in self.trackers.items() if t.stage == "fixed"}
         out = exchange_clip_results(dict(zip(mine, own)), lengths, list(self.trackers), fixed)
         self.timings["_clips_exchange"] = timeit.default_timer() - t0
         das = None
@@ -813,19 +788,18 @@ class TrackingRunner:
         from .ball_tracker import median_background_device
 
         ids = list(range(len(srcs))) if clip_ids is None else list(clip_ids)
-        fixed = {n: t for n, t in self.trackers.items() if getattr(t, "fixed_keypoints_detection", None) is not None}
-        model = {n: t for n, t in self.trackers.items() if n not in fixed and (
-            isinstance(t, (PlayerTracker, PlayerKeypointsTracker, BallTracker)) or
-            (isinstance(t, KeypointsTracker) and t.model is not None))}
+        fixed = {n: t for n, t in self.trackers.items() if t.stage == "fixed"}
+        model = _batch_trackers(self.trackers)
         other = set(self.trackers) - set(fixed) - set(model)
         if other:
-            raise ValueError(f"run_clips: trackers {sorted(other)} have neither a model nor a fixed detection")
-        out = [{n: [t.fixed_keypoints_detection] * T for n, t in fixed.items()} for T in lengths]
+            raise ValueError(f"run_clips: trackers {sorted(other)} have no batch model stage (a YOLO or ball model) "
+                             "and no fixed detection")
+        out = [{n: [t.fixed_detection] * T for n, t in fixed.items()} for T in lengths]
         if not model or not sum(lengths):
             for res, T in zip(out, lengths):
                 res.update({n: [] for n in model})
             return out, hw
-        ball_name, ball = next(((n, t) for n, t in model.items() if isinstance(t, BallTracker)), (None, None))
+        ball_name, ball = next(((n, t) for n, t in model.items() if t.stage == "ball"), (None, None))
         B = min(t.batch_size for t in model.values())
         side = torch.cuda.Stream()  # backgrounds of the clips ahead are computed beside the pass
         meds: dict = {}
@@ -869,9 +843,7 @@ class TrackingRunner:
             """InpaintNet over the clip's trajectory (on a stream of its own: the pass keeps running) -> Ball list"""
             ball.video_info = infos[c]
             with torch.cuda.stream(inpaint_stream):
-                v = ball.inpaint_xyv(xyv[c], lengths[c])
-            out[c][ball_name] = [Ball(frame=n, xy=(v[n][0], v[n][1]), visibility=v[n][2]) if n in v
-                                 else Ball(frame=n, xy=(0.0, 0.0), visibility=0) for n in range(lengths[c])]
+                out[c][ball_name] = ball.balls(xyv[c], lengths[c])
 
         for res in fp.run(itertools.chain([first], gen)):
             for name, parts in res.items():
@@ -921,19 +893,8 @@ class BallRecords:
 
 
 def _yolo_records(blocks: list, tracker) -> YoloRecords:
-    """This rank's frames (a list of per-batch ResultBlocks, or of Results) as one padded block."""
+    """This rank's frames (a list of per-batch ResultBlocks) as one padded block."""
     kpt_shape = tracker.model.kpt_shape
-    if blocks and not isinstance(blocks[0], ResultBlock):  # plain Results: one frame each
-        rowlen = 6 + (kpt_shape[0] * kpt_shape[1] if kpt_shape else 0)
-        one = []
-        for r in blocks:
-            n = len(r.boxes)
-            rows = np.zeros((1, max(n, 1), rowlen), dtype=np.float32)
-            rows[0, :n, :6] = r.boxes.data.numpy()
-            if kpt_shape and n:
-                rows[0, :n, 6:] = r.keypoints.data.numpy().reshape(n, rowlen - 6)
-            one.append(ResultBlock(rows, np.array([n], dtype=np.int32), kpt_shape, r.names, r.orig_shape))
-        blocks = one
     rowlen = 6 + (kpt_shape[0] * kpt_shape[1] if kpt_shape else 0)
     empty = ResultBlock(np.zeros((0, 1, rowlen), np.float32), np.zeros((0,), np.int32), kpt_shape, None, None)
     blk = ResultBlock.concat(blocks, like=empty)

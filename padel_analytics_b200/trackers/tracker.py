@@ -77,6 +77,13 @@ def sampler(generator: Iterable[np.ndarray], sequence_length: int):
 
 class Tracker(ABC):
     batch_size: int
+    # How TrackingRunner drives the tracker:
+    #   "ball"   -- windows streamed through BallTracker's device pipeline (stream_begin / stream_push_async)
+    #   "detect" -- detect_sample_async(batch), then postprocess(results, frame_hw), the order-dependent host stage
+    #   "fixed"  -- `fixed_detection` repeated for every frame
+    #   "frames" -- predict_and_update only
+    stage: str = "frames"
+    fixed_detection: Optional[Object] = None
 
     def __init__(self, load_path: Optional[str | Path] = None, save_path: Optional[str | Path] = None) -> None:
         self.results = TrackingResults()
@@ -121,6 +128,10 @@ class Tracker(ABC):
 
     def to(self, device: str) -> None:
         pass
+
+    def detect_sample(self, sample):
+        """A "detect" tracker's model stage on one sample: the engine's raw results, no sequential state."""
+        return self.detect_sample_async(sample)()
 
     @abstractmethod
     def predict_sample(self, sample: Iterable[np.ndarray], **kwargs): ...

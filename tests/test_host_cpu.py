@@ -145,6 +145,50 @@ def test_runner_single_process():
     assert t.results.predictions == list(range(10))
 
 
+def _stub(cls, **attrs):
+    t = object.__new__(cls)  # no CUDA here: skip the engine construction, set what is read
+    for k, v in attrs.items():
+        setattr(t, k, v)
+    return t
+
+
+def test_tracker_stages():
+    """Each tracker declares how TrackingRunner drives it: "detect" (YOLO model), "fixed", "ball" or "frames"."""
+    from padel_analytics_b200.trackers import BallTracker, KeypointsTracker, PlayerKeypointsTracker, PlayerTracker
+
+    def kt(**kw):
+        return _stub(KeypointsTracker, **{"model_type": "yolo", "model": object(), "fixed_keypoints_detection": None,
+                                          **kw})
+
+    court = Keypoints([Keypoint(id=0, xy=(1.0, 2.0))])
+    cases = [(_stub(PlayerTracker), "detect", None), (_stub(PlayerKeypointsTracker), "detect", None),
+             (kt(), "detect", None), (kt(fixed_keypoints_detection=court), "fixed", court),
+             (kt(model=None, fixed_keypoints_detection=court), "fixed", court), (kt(model=None), "frames", None),
+             (kt(model_type="resnet"), "frames", None), (_stub(BallTracker), "ball", None), (_Echo(), "frames", None)]
+    for t, stage, fixed in cases:
+        assert (t.stage, t.fixed_detection) == (stage, fixed), (type(t).__name__, vars(t))
+
+
+def test_runner_runs_frames_stage_trackers_in_frame_order():
+    """Two trackers of stage "frames" (the echo, and a ResNet court regressor -- here a CPU stand-in for the engine)
+    run through predict_and_update; both hold one result per frame, in frame order."""
+    from types import SimpleNamespace
+
+    from padel_analytics_b200.trackers import KeypointsTracker
+
+    def regress(chunk):  # (n, 24) in [0, 1]: frame i -> every coordinate i / 16
+        return np.array([[f[0, 0, 0] / 16.0] * 24 for f in chunk], dtype=np.float32)
+
+    echo = _Echo()
+    kt = KeypointsTracker(None, batch_size=4, model_type="yolo")
+    kt.model_type, kt.model = "resnet", SimpleNamespace(predict_frames=regress, to=lambda device: None)
+    assert (echo.stage, kt.stage) == ("frames", "frames")
+    R.TrackingRunner([echo, kt]).run(frame_source=_frames, total_frames=10)
+    assert echo.results.predictions == list(range(10))
+    assert [[k.xy for k in p.keypoints] for p in kt.results.predictions] == [[(i / 8, i / 8)] * 12 for i in range(10)]
+    assert [[k.id for k in p.keypoints] for p in kt.results.predictions] == [list(range(12))] * 10
+
+
 def test_runner_world2_gloo(tmp_path):
     """Two processes over gloo: each handles its contiguous shard, rank 0 assembles frame-ordered results."""
     script = tmp_path / "w.py"
@@ -171,42 +215,50 @@ dist.destroy_process_group()
     assert "WORLD2_OK" in r.stdout, r.stdout + r.stderr
 
 
-def _fake_results(frames, kpt_shape, seed=0):
-    """Deterministic ragged per-frame Results (0..5 detections) keyed by absolute frame number."""
-    from padel_analytics_b200.engine.yolo_engine import Boxes, Keypoints, Result
+def _fake_blocks(frames, kpt_shape, seed=0, per_block=4):
+    """Deterministic ragged detections (0..5 per frame) keyed by absolute frame number, as the per-batch ResultBlocks
+    of a pass: `per_block` frames each, the last block partial."""
+    from padel_analytics_b200.engine.yolo_engine import ResultBlock
 
+    frames = list(frames)
+    rowlen = 6 + (kpt_shape[0] * kpt_shape[1] if kpt_shape else 0)
     out = []
-    for n in frames:
-        g = torch.Generator().manual_seed(1000 * seed + n)
-        k = int(torch.randint(0, 6, (1,), generator=g))
-        box = torch.rand((k, 6), generator=g) * 100 + n
-        kp = None
-        if kpt_shape:
-            kp = Keypoints(torch.rand((k,) + tuple(kpt_shape), generator=g) * 50 + n)
-        out.append(Result(Boxes(box), kp, {0: "x"}, None))
+    for i in range(0, len(frames), per_block):
+        chunk = frames[i:i + per_block]
+        rows = np.zeros((len(chunk), 5, rowlen), np.float32)
+        counts = np.zeros((len(chunk),), np.int32)
+        for j, n in enumerate(chunk):
+            g = torch.Generator().manual_seed(1000 * seed + n)
+            k = int(torch.randint(0, 6, (1,), generator=g))
+            rows[j, :k, :6] = (torch.rand((k, 6), generator=g) * 100 + n).numpy()
+            if kpt_shape:
+                kp = torch.rand((k,) + tuple(kpt_shape), generator=g) * 50 + n
+                rows[j, :k, 6:] = kp.reshape(k, rowlen - 6).numpy()
+            counts[j] = k
+        out.append(ResultBlock(rows, counts, kpt_shape, {0: "x"}, None))
     return out
 
 
-def test_runner_world2_gloo_fixed_capacity_records(tmp_path):
-    """The sharded gather of SURVEY 8(e): ragged per-frame detections -> padded (frames, cap, 6+K*D) blocks + counts,
-    all_gather over gloo, rank 0 rebuilds the frame-ordered Results; ball (x, y, vis) int32 records likewise."""
+def test_runner_world2_gloo_fixed_capacity_block_records(tmp_path):
+    """The sharded gather of SURVEY 8(e): ragged per-batch detection blocks -> padded (frames, cap, 6+K*D) blocks +
+    counts, all_gather over gloo, rank 0 rebuilds the frame-ordered Results; ball (x, y, vis) int32 records likewise."""
     script = tmp_path / "w2.py"
     script.write_text(f"""
 import sys
 sys.path.insert(0, {str(ROOT)!r}); sys.path.insert(0, {str(ROOT / 'tests')!r})
 import torch, torch.distributed as dist
 from types import SimpleNamespace
-from test_host_cpu import _fake_results
+from test_host_cpu import _fake_blocks
 from padel_analytics_b200.trackers import runner as R
 dist.init_process_group('gloo')
 rank, world, total = dist.get_rank(), dist.get_world_size(), 23
 lo, hi = R.shard_range(total, rank, world)
 for kpt_shape in (None, (13, 3)):
     trk = SimpleNamespace(model=SimpleNamespace(kpt_shape=kpt_shape, names={{0: 'x'}}))
-    rec = R._yolo_records(_fake_results(range(lo, hi), kpt_shape), trk)
+    rec = R._yolo_records(_fake_blocks(range(lo, hi), kpt_shape), trk)
     parts = R._all_gather_yolo(rec, total, rank, world)
     got = [r for p in parts for r in p.to_results(trk)]
-    exp = _fake_results(range(total), kpt_shape)
+    exp = [r for b in _fake_blocks(range(total), kpt_shape) for r in b]
     assert len(got) == total
     for g, e in zip(got, exp):
         assert torch.equal(g.boxes.data, e.boxes.data)

@@ -188,6 +188,33 @@ def test_runner_computes_the_background_median_on_device_when_none_is_given():
     assert bt.track_xyv(iter(fr), T) == a
 
 
+@pytest.mark.parametrize("fused", [None, True, False])
+def test_runner_drives_the_resnet_court_regressor_through_predict_frames(fused):
+    """KeypointsTracker(model_type="resnet") has no batch model stage (the reference runs it through predict_frames):
+    run(), fused or not, gives it the keypoints of predict_and_update alone, and the player tracker beside it the
+    results of a run of its own; run_clips refuses it with a ValueError naming it."""
+    from oracle import resnet as OR
+
+    T, B = 5, 2
+    fr = [f.numpy() for f in synth.make_frames(T, H, W, start=4)]
+    src = lambda lo, hi: iter(fr[lo:hi])
+    sd = OR.make_resnet50_court()
+    ck = OW.make_yolo("detect")
+    poly = sv.PolygonZone(np.array([[0, 0], [W - 1, 0], [W - 1, H - 1], [0, H - 1]]), frame_resolution_wh=(W, H))
+    alone = KeypointsTracker(sd, batch_size=B, model_type="resnet")
+    alone.predict_and_update(iter(fr))
+    pt_alone = PlayerTracker(ck, poly, batch_size=B)
+    TrackingRunner([pt_alone], video_info=_vi(T)).run(frame_source=src, total_frames=T)
+    kt = KeypointsTracker(sd, batch_size=B, model_type="resnet")
+    pt = PlayerTracker(ck, poly, batch_size=B)
+    run = TrackingRunner([pt, kt], video_info=_vi(T))
+    run.run(frame_source=src, total_frames=T, fused=fused)
+    assert _dump([kt]) == _dump([alone]) and _dump([pt]) == _dump([pt_alone])
+    assert len(kt.results) == len(pt.results) == T
+    with pytest.raises(ValueError, match="keypoints_tracker"):
+        run.run_clips([(src, T)])
+
+
 def test_runner_sharded_over_nccl_equals_unsharded(tmp_path):
     """World-size-2 NCCL run of TrackingRunner.run (contiguous shards, ball halo, broadcast median, fixed-capacity
     all_gather, rank-0 ByteTrack/objects) == the single-process run.  Needs two GPUs (`gpurun --gpus 2`)."""
