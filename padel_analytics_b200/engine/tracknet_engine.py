@@ -168,11 +168,47 @@ class TrackNetEngine:
         return self._pred_new[:nb].clone()
 
 
+def window_desc(w0: int, nb: int, total_frames: int | None) -> np.ndarray:
+    """Ensemble descriptors (window 0, window count, frame) of the frames a batch of windows [w0, w0+nb) of one video
+    emits: frame w per window w, plus the 7 tail frames (ball_tracker.py:486-509) when the batch runs the video's last
+    window.  total_frames=None: the video's end is not known yet (a stream), so the batch emits its windows' own
+    frames only, with w0 + nb as their window count.  Any count above a frame selects the same rule for it (head
+    below frame 7, else the weighted sum of windows n-7..n) as the true count, which is larger still."""
+    tw = w0 + nb if total_frames is None else total_frames - 7
+    nframes = nb + (7 if total_frames is not None and w0 + nb == tw else 0)
+    desc = np.zeros((nframes, 3), dtype=np.int32)
+    desc[:, 1] = tw
+    desc[:, 2] = np.arange(w0, w0 + nframes)
+    return desc
+
+
+def tail_desc(total_frames: int) -> np.ndarray:
+    """Descriptors of the 7 tail frames of a video of `total_frames` >= 8 frames, for a launch that runs no window:
+    the stream's last window already ran while its end was unknown, and the 7-window carry still holds the windows
+    these frames read (ball_tracker.py:486-509: frame T-8+i, i = 1..7, is the mean of the 8-i windows that hold it)."""
+    tw = total_frames - 7
+    desc = np.zeros((7, 3), dtype=np.int32)
+    desc[:, 1] = tw
+    desc[:, 2] = np.arange(tw, total_frames)
+    return desc
+
+
+def ready_batches(next_window: int, frames_end: int, B: int, total_frames: int | None) -> list[tuple[int, int]]:
+    """(first window, window count) of the batches of up to B windows that run every window computable now: window w
+    needs frames w..w+7, so the windows [next_window, frames_end - 7) are ready (frames_end: one past the last frame
+    that arrived), capped at the video's last window when `total_frames` is known."""
+    end = frames_end - 7 if total_frames is None else min(frames_end, total_frames) - 7
+    return [(w, min(B, end - w)) for w in range(next_window, end, B)]
+
+
 class BallPipeline:
     """Frames (BGR u8) -> per-frame ball bbox, entirely on device: PIL-exact resize, window packing, TrackNet,
     temporal ensemble + threshold, connected components.  Mirrors BallTracker.predict_frames' TrackNet stage
     (ball_tracker.py:373-523) including its head/tail ensemble rules (SURVEY App. C).  One video: its background is
-    slot 0 of a one-slot median pool, and its windows are numbered from 0 as the one clip of the batch tables."""
+    slot 0 of a one-slot median pool, and its windows are numbered from 0 as the one clip of the batch tables.
+
+    The video's length may be unknown while frames arrive (a stream): the launches then emit only frames whose
+    ensemble does not depend on where the video ends, and `stream_end` emits the 7 tail frames once it is known."""
 
     def __init__(self, engine: TrackNetEngine, frame_hw: tuple[int, int], median_rgb: np.ndarray | torch.Tensor):
         self._init_buffers(engine, frame_hw, ring=engine.B + 8, pool=1, max_frames=engine.B + 7)
@@ -229,6 +265,7 @@ class BallPipeline:
         self.base = base
         self.n_frames_in = 0  # frames received
         self.n_windows = 0  # windows processed
+        self.tail_emitted = False  # the launch of the video's last window emitted its 7 tail frames
         self.eng.pred.zero_()
 
     def _resize(self, src, n, dst_f16, swap_rb):
@@ -259,39 +296,50 @@ class BallPipeline:
     def windows_ready(self) -> int:
         return max(0, self.n_frames_in - 7) - self.n_windows
 
-    def run_windows(self, nb: int, total_frames: int, want_ens: bool = False):
+    def run_windows(self, nb: int, total_frames: int | None, want_ens: bool = False):
         """Process the next nb windows (nb <= B). Returns (first_frame, host int32 (nframes,4) bboxes) for the frames
         emitted: absolute frames [first_frame, first_frame+nframes)."""
         return self.run_windows_async(nb, total_frames, want_ens)()
 
-    def run_windows_async(self, nb: int, total_frames: int, want_ens: bool = False):
+    def run_windows_async(self, nb: int, total_frames: int | None, want_ens: bool = False):
         """Enqueue the device work for the next nb windows; returns a callable that waits and yields
-        (first_frame, bboxes).  One call in flight."""
+        (first_frame, bboxes).  One call in flight.  total_frames=None: the video's length is not known yet
+        (`window_desc`)."""
         assert 0 < nb <= self.B and nb <= self.windows_ready()
         w0 = self.base + self.n_windows  # absolute window index
-        total_windows = total_frames - 7
-        if w0 + nb > total_windows:
+        if total_frames is not None and w0 + nb > total_frames - 7:
             raise L.PbError("BallPipeline: more windows than total_frames allows")
-        nframes = nb + (7 if w0 + nb == total_windows else 0)
-        desc = np.zeros((nframes, 3), dtype=np.int32)  # the video is one clip whose window 0 is window 0
-        desc[:, 1] = total_windows
-        desc[:, 2] = np.arange(w0, w0 + nframes)
+        desc = window_desc(w0, nb, total_frames)  # the video is one clip whose window 0 is window 0
         fin = self._launch_batch(w0, w0, (self.n_windows + np.arange(nb)) % self.ring, np.zeros(nb), desc, want_ens)
         self.n_windows += nb
+        self.tail_emitted = len(desc) > nb
         return fin
 
-    def run_ready_async(self, total_frames: int) -> list:
-        """Enqueue every window that has become computable, in batches of up to B, with at most one launch in flight
-        (each launch is waited for before the next is enqueued).  Returns the launches' finish callables in order."""
+    def run_ready_async(self, total_frames: int | None) -> list:
+        """Enqueue every window that has become computable (`ready_batches`), in batches of up to B, with at most one
+        launch in flight (each launch is waited for before the next is enqueued).  Returns the launches' finish
+        callables in order."""
         fins = []
-        while True:
-            nb = min(self.B, self.windows_ready(), total_frames - 7 - (self.base + self.n_windows))
-            if nb <= 0:
-                return fins
+        for _, nb in ready_batches(self.base + self.n_windows, self.base + self.n_frames_in, self.B, total_frames):
             if fins:
                 res = fins[-1]()
                 fins[-1] = lambda res=res: res
             fins.append(self.run_windows_async(nb, total_frames))
+        return fins
+
+    def stream_end(self, total_frames: int) -> list:
+        """The video ends at frame `total_frames`, the last frame pushed.  Enqueues the windows not run yet, whose last
+        batch emits the 7 tail frames, or, when the last window already ran while the end was unknown, a launch of no
+        window that emits the tail from the 7 windows carried in the heat-map buffer.  Returns the launches' finish
+        callables in order, as `run_ready_async` does."""
+        if self.base + self.n_frames_in != total_frames:
+            raise L.PbError(f"BallPipeline: stream_end({total_frames}) after {self.base + self.n_frames_in} frames")
+        fins = self.run_ready_async(total_frames)
+        if total_frames >= 8 and not self.tail_emitted:
+            tw = total_frames - 7
+            fins.append(self._launch_batch(tw, tw, np.zeros(0), np.zeros(0), tail_desc(total_frames)))
+            self.tail_emitted = True
+        return fins
 
     def _launch_batch(self, key, first_window: int, row_slot, row_median, desc, want_ens: bool = False):
         """Enqueue one batch of nb = len(row_slot) windows: pack, TrackNet, ensemble + threshold, boxes, download.
@@ -323,10 +371,11 @@ class BallPipeline:
         t[:nb], t[nb:2 * nb], t[2 * nb:n] = row_slot, row_median, desc.reshape(-1)
         self._tables[:n].copy_(stage[:n], non_blocking=True)
         rows = self._tables.data_ptr()
-        L.check(L.lib().pb_tracknet_pack_windows_rows(self.small.data_ptr(), self.ring, rows, self.medians.data_ptr(),
-                                                      rows + 4 * nb, nb, eng.H, eng.W, eng.x.data_ptr(),
-                                                      L.stream_ptr()))
-        eng.run_packed()
+        if nb:  # nb = 0: a stream's tail, ensembled from the carried windows alone
+            L.check(L.lib().pb_tracknet_pack_windows_rows(self.small.data_ptr(), self.ring, rows,
+                                                          self.medians.data_ptr(), rows + 4 * nb, nb, eng.H, eng.W,
+                                                          eng.x.data_ptr(), L.stream_ptr()))
+            eng.run_packed()
         ens_ptr = None
         if want_ens:
             self.ens = torch.empty((nframes, eng.H, eng.W), dtype=torch.float32, device=self.dev)
@@ -339,8 +388,9 @@ class BallPipeline:
             L.check(L.lib().pb_ccl_bbox(self.mask[f:].data_ptr(), m, eng.H, eng.W, self.scratch.data_ptr(),
                                         self.bbox[f:].data_ptr(), L.stream_ptr()))
         # carry the last 7 windows for the next batch (ball_tracker.py:523), which may start another clip
-        carry = eng.pred[nb:nb + 7].clone()
-        eng.pred[:7].copy_(carry)
+        if nb:
+            carry = eng.pred[nb:nb + 7].clone()
+            eng.pred[:7].copy_(carry)
         host = self._host_ring[slot]
         host[:nframes].copy_(self.bbox[:nframes], non_blocking=True)
         done = torch.cuda.Event()

@@ -198,7 +198,12 @@ class BallTracker(Tracker):
         return out
 
     # ---- streaming interface used by the fused single-pass runner (one batch at a time, device work asynchronous) ----
-    def stream_begin(self, frame_hw, total_frames: int, first_frame: int = 0, emit_range=None, median=None):
+    def stream_begin(self, frame_hw, total_frames: Optional[int] = None, first_frame: int = 0, emit_range=None,
+                     median=None):
+        """Start a stream of frames first_frame, first_frame+1, ... through the device pipeline.  total_frames=None:
+        the stream's length is unknown until `stream_end_async`; until then each push emits only the frames whose
+        result cannot depend on where the stream ends (frame f once frame f+7 has arrived).  median: (H,W,3) uint8
+        RGB background, host or device (defaults to `self.median`)."""
         median = self.median if median is None else median
         if median is None:
             raise ValueError("stream_begin needs a background median (pass median= to BallTracker or here)")
@@ -267,6 +272,14 @@ class BallTracker(Tracker):
         fin = self._xyv_finish(pipe.run_ready_async(s["total"]), itertools.count)  # a launch yields its first frame
         emit = s["emit"]
         return lambda: {n: v for n, v in fin() if emit is None or emit[0] <= n < emit[1]}
+
+    def stream_end_async(self, total_frames: int):
+        """End a stream begun without a total at frame `total_frames` (every frame has been pushed): enqueues the
+        last windows and the 7 tail frames (`BallPipeline.stream_end`); returns a callable that waits and yields
+        {frame: (x, y, vis)} for the frames not emitted yet."""
+        self._stream["total"] = total_frames
+        fin = self._xyv_finish(self._pipe.stream_end(total_frames), itertools.count)
+        return lambda: dict(fin())
 
     # ---- InpaintNet stage (ball_tracker.py:525-673) -------------------------------------------------------------
     @staticmethod

@@ -2,8 +2,9 @@
 
 A frame source is a callable `src(lo, hi)` that yields frames lo..hi-1 of a video, either as HWC uint8 BGR numpy
 frames (video decode) or as ready uint8 (n,H,W,3) batches: host tensors (pinned or not) or device tensors.  `read`
-turns either into (n,H,W,3) tensors, `chunks` packs those into upload batches, and `head` splits off the first frames
-(the ball tracker's background median).
+turns either into (n,H,W,3) tensors (`tensors` does so for any iterable, such as a stream of unknown length),
+`chunks` packs those into upload batches, and `head` splits off the first frames (the ball tracker's background
+median).
 """
 from __future__ import annotations
 
@@ -24,15 +25,7 @@ def read(src: Callable, lo: int, hi: int, hw: Optional[tuple[int, int]] = None, 
     want, seen = hi - lo, 0
     if want <= 0:
         return
-    for item in src(lo, hi):
-        t = item if isinstance(item, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(item))
-        if t.dim() == 3:
-            t = t.unsqueeze(0)
-        if hw is None:
-            hw = tuple(t.shape[1:3])
-        if tuple(t.shape[1:3]) != tuple(hw):
-            raise ValueError(f"clip {clip} has {tuple(t.shape[1:3])} frames, not {tuple(hw)}: all frames of one call "
-                             "must have the same frame size")
+    for t in tensors(src(lo, hi), hw, f"clip {clip}"):
         t = t[:want - seen]
         seen += t.shape[0]
         if t.shape[0]:
@@ -41,6 +34,23 @@ def read(src: Callable, lo: int, hi: int, hw: Optional[tuple[int, int]] = None, 
             return
     if exact:
         raise ValueError(f"clip {clip} yielded {seen} frames, {want} announced")
+
+
+def tensors(items: Iterable, hw: Optional[tuple[int, int]] = None, what: str = "the stream"
+            ) -> Iterator[torch.Tensor]:
+    """HWC uint8 BGR frames or (n,H,W,3) batches (host or device) as (n,H,W,3) tensors, one per item, pulled one at a
+    time: an HWC array is wrapped without a copy and gets a leading axis.  Every item must have the frame size `hw`
+    (default: that of the first item), else ValueError naming `what`."""
+    for item in items:
+        t = item if isinstance(item, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(item))
+        if t.dim() == 3:
+            t = t.unsqueeze(0)
+        if hw is None:
+            hw = tuple(t.shape[1:3])
+        if tuple(t.shape[1:3]) != tuple(hw):
+            raise ValueError(f"{what} has {tuple(t.shape[1:3])} frames, not {tuple(hw)}: all frames of one call "
+                             "must have the same frame size")
+        yield t
 
 
 def _pinned(shape: tuple) -> torch.Tensor:

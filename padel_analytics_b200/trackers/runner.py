@@ -8,7 +8,8 @@ renders the annotated video to `inference_path` and collects the players' court 
 `pb_render_overlay`) and encoding runs on a thread of its own.  `run_clips()` does the same per clip for a list of
 clips.  Both draw through one render pass over clips played back to back (`_render_clips`; `run()`'s video is one
 clip).  Under torch.distributed `run_clips()` shards whole clips over the ranks (`plan_clip_shards`) and exchanges the
-results once after the pass.
+results once after the pass.  `stream()` tracks an iterable of frames of unknown length (a live feed) and yields each
+frame's results as soon as every tracker has them (`FrameMerge`).
 
 Documented deviations from reference quirks (SURVEY App. E):
   q7  with collect_data=False the reference's drawing pass ends by trimming `self.data_analytics.frames`, which is
@@ -18,11 +19,12 @@ Documented deviations from reference quirks (SURVEY App. E):
 """
 from __future__ import annotations
 
+import collections
 import contextlib
 import itertools
 import os
 import timeit
-from typing import Callable, Iterable, Optional
+from typing import Callable, Iterable, Iterator, Optional
 
 import numpy as np
 import torch
@@ -85,13 +87,16 @@ class FusedPass:
     are SMs — so three independent chains fill the machine), the ball tracker after them on the caller's stream;
     2 = all trackers concurrent.  The kernels and their inputs are the same in every mode, so are the results."""
 
-    def __init__(self, trackers: dict[str, Tracker], frame_hw: tuple[int, int], batch_size: int, total_frames: int,
-                 first_frame: int = 0, emit_range: Optional[tuple[int, int]] = None, streams: Optional[int] = None,
-                 raw: bool = False, median=None):
+    def __init__(self, trackers: dict[str, Tracker], frame_hw: tuple[int, int], batch_size: int,
+                 total_frames: Optional[int], first_frame: int = 0, emit_range: Optional[tuple[int, int]] = None,
+                 streams: Optional[int] = None, raw: bool = False, median=None):
         """raw=True: the YOLO trackers' entries are the engines' raw per-frame Results (no polygon filter / ByteTrack /
         result objects) -- what a shard hands to rank 0, where the order-dependent host stages run once over the
-        ordered gather.  median: background for the ball tracker (defaults to BallTracker.median)."""
+        ordered gather.  median: background for the ball tracker (defaults to BallTracker.median).
+        total_frames=None: a stream whose length is known only when `run`'s batches end; `run` then ends with one
+        more entry, the ball tracker's last windows and tail frames."""
         self.trackers = trackers
+        self.total = total_frames
         self.raw = raw
         self.mode = int(os.environ.get("PADEL_B200_STREAMS", "1")) if streams is None else streams
         # side streams: the YOLO chains at high priority (their CTAs are placed first whenever SMs free up), the ball
@@ -180,13 +185,19 @@ class FusedPass:
 
         One batch of look-ahead: batch i+1 is pulled from `batches` and enqueued before batch i's results are yielded.
         A batch (host pieces: copied asynchronously into a staging slot; one device tensor: read in place) must stay
-        untouched until ITS OWN results have been yielded, i.e. a producer that reuses buffers needs at least two."""
+        untouched until ITS OWN results have been yielded, i.e. a producer that reuses buffers needs at least two.
+
+        Without a total (a stream), the ball tracker emits a frame once the frame 7 later has been pushed, and after
+        the last batch's dict comes one more, {ball tracker name: results of the last frames} (`_end`)."""
         it = iter(batches)
         main = torch.cuda.current_stream()
+        pushed = 0
 
         def start(batch, i):
             """upload (copy stream) + enqueue all device work of batch i; returns the launch record"""
+            nonlocal pushed
             dev = self._upload(batch, i % 2)
+            pushed += dev.shape[0]
             staged = dev.data_ptr() == self.staging[i % 2].data_ptr()
             if staged:
                 main.wait_event(self.ready[i % 2])
@@ -208,6 +219,13 @@ class FusedPass:
             nrec = start(nxt, i + 1) if nxt is not None else None
             yield self._finish(rec)
             rec, i = nrec, i + 1
+        if self.total is None:
+            yield self._end(pushed)
+
+    def _end(self, total: int) -> dict:
+        """The last step of a stream of `total` frames: the ball tracker's last windows and its 7 tail frames.  They
+        are enqueued on the caller's stream, which every tracker's stream has joined after each batch."""
+        return {name: t.stream_end_async(total)() for name, t in self.trackers.items() if t.stage == "ball"}
 
 
 class ClipPass(FusedPass):
@@ -257,6 +275,34 @@ class ClipPass(FusedPass):
                     t.video_info_post_init(self.clip_infos[c])
                 parts.append((c, t.postprocess(res[a:b], self.hw)))
             out[name] = parts
+        return out
+
+
+class FrameMerge:
+    """In-order merge of per-tracker results for `TrackingRunner.stream`.  Each tracker's results arrive in frame
+    order, but the trackers are out of step with one another: a YOLO tracker has a batch's frames when the batch is
+    done, the ball tracker has them 7 frames later.  `put` hands over one tracker's result for its next frame; `ready`
+    pops, in frame order, every frame that all trackers have."""
+
+    def __init__(self, names: Iterable[str]):
+        self.held = {n: collections.deque() for n in names}
+        if not self.held:
+            raise ValueError("FrameMerge needs at least one tracker")
+        self.next = {n: 0 for n in self.held}  # per tracker: the frame its next result is for
+        self.frame = 0  # the next frame `ready` pops
+
+    def put(self, name: str, frame: int, obj) -> None:
+        if frame != self.next[name]:
+            raise ValueError(f"{name}: a result for frame {frame}, but frame {self.next[name]} is next")
+        self.held[name].append(obj)
+        self.next[name] += 1
+
+    def ready(self) -> list[tuple[int, dict]]:
+        """[(frame, {tracker name: result})] of the frames every tracker has now, in frame order."""
+        out = []
+        for f in range(self.frame, min(self.next.values())):
+            out.append((f, {n: q.popleft() for n, q in self.held.items()}))
+        self.frame = max(self.frame, min(self.next.values()))
         return out
 
 
@@ -373,6 +419,139 @@ class TrackingRunner:
             if rank == 0:
                 tracker.save_predictions()
         return self.timings
+
+    # ---- a frame stream of unknown length -------------------------------------------------------------------------
+    def stream(self, frames_in: Iterable, median=None) -> Iterator[tuple[int, dict]]:
+        """Track a stream of frames whose length is not known in advance (a camera, a broadcast, a long recording):
+        a generator of `(frame index, {tracker name: Object})` in frame order, each frame yielded as soon as every
+        tracker's result for it is final.
+
+        frames_in: any iterable of HWC uint8 BGR frames or uint8 (n,H,W,3) batches, host or device; the stream ends
+        when the iterable does.  Every frame must have the size of the first (ValueError).  Host frames that are not
+        pinned are copied as they are pulled; a pinned or device batch is read in place and must stay untouched until
+        its frames have been yielded.  The fps (ByteTrack) and the frame size that scales the ball's coordinates come
+        from the runner's `video_info`.
+
+        Trackers of stage "detect", "ball" and "fixed" are supported.  A "frames" tracker (the ResNet court regressor),
+        a tracker holding cached predictions (a stream has no frame count to match them against) and a torch.distributed
+        job of world size > 1 are refused with ValueError, before any frame is pulled.
+
+        Results: while the stream runs, each tracker's `results.predictions` grows by the frames yielded.  The Ball
+        yielded per frame is TrackNet's: InpaintNet needs the whole trajectory, so when the stream ends the ball
+        tracker's `results` are replaced by `balls(trajectory, frame count)`, which applies InpaintNet.  Then every
+        tracker's `results` equal what `run()` gives on the same frames, and, as after `run()`, the model trackers
+        are moved to the CPU and every tracker with a `save_path` writes its predictions.  A caller that stops early
+        keeps the results of the frames yielded, without InpaintNet, and nothing is saved.
+
+        Unlike `run()`, which switches Python's cyclic garbage collector off for its pass, `stream` leaves it as the
+        caller set it: a generator cannot switch it off for its own steps without switching it off for the caller's
+        code between them.  The results kept per frame are many small objects that form no cycles, so on a long
+        stream each full collection walks more of them; a caller for whom those pauses matter can call
+        `gc.disable()` (or `gc.freeze()`) around its loop.
+
+        Background: `median` ((H,W,3) uint8 RGB), else `BallTracker.median`, else the median of the stream's first
+        `median_max_sample_num` frames (`run()`'s background), which are held on the device until it is computed.  No
+        frame is yielded before the background exists, so that every tracker's entries stay in frame order.
+
+        Latency: with B the pass's batch (the smallest batch_size of the "detect" and "ball" trackers), the entry of
+        frame f is yielded before the pass pulls frame f + 2B + 8 from `frames_in` (one batch in flight, one batch of
+        look-ahead, the 7 frames the ball ensemble looks ahead), for every f whose frame f + 2B + 8 comes after the
+        frames held for the background.  An item of n frames is pulled whole, which moves the bound by up to n - 1
+        frames.  A live caller picks a small batch_size."""
+        import torch.distributed as dist
+
+        if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+            raise ValueError(f"stream: a stream runs in one process, not over a torch.distributed job of world size "
+                             f"{dist.get_world_size()}")
+        if not self.trackers:
+            raise ValueError("stream: no trackers")
+        other = sorted(n for n, t in self.trackers.items() if t.stage not in ("detect", "ball", "fixed"))
+        if other:
+            raise ValueError(f"stream: trackers {other} have no batch model stage (a YOLO or ball model) and no fixed "
+                             "detection")
+        cached = sorted(n for n, t in self.trackers.items() if len(t))
+        if cached:
+            raise ValueError(f"stream: trackers {cached} hold cached predictions, and a stream has no frame count to "
+                             "match them against (restart() them first)")
+        if self.video_info is None:
+            raise ValueError("stream: the fps and the ball's frame size come from video_info, and this runner has none")
+        return self._stream(frames_in, median)
+
+    def _stream(self, frames_in: Iterable, median) -> Iterator[tuple[int, dict]]:
+        from .ball_tracker import median_background_device
+
+        model = _batch_trackers(self.trackers)
+        fixed = {n: t.fixed_detection for n, t in self.trackers.items() if t.stage == "fixed"}
+        ball_name, ball = next(((n, t) for n, t in model.items() if t.stage == "ball"), (None, None))
+        merge = FrameMerge(self.trackers)
+        pieces = frames.tensors(frames_in)
+        if ball is not None:
+            median = ball.median if median is None else median
+            if median is None:  # iterable.py:58-73, as run() does: the first frames, copied as they are pulled
+                m, held = ball.median_max_sample_num, [0]
+
+                def own(p):
+                    keep = held[0] < m
+                    held[0] += p.shape[0]
+                    return p.to("cuda", copy=True) if keep else p
+
+                first, pieces = frames.head(map(own, pieces), m)
+                if held[0]:
+                    median = median_background_device(first)
+                pieces = itertools.chain(first, pieces)
+        if model:
+            B = min(t.batch_size for t in model.values())
+            for t in model.values():
+                t.to(t.DEVICE)
+            sizes = collections.deque()  # frames of each chunk the pass has pulled and not yet finished
+
+            def sized(chunks):
+                for c in chunks:
+                    sizes.append(sum(p.shape[0] for p in c))
+                    yield c
+
+            chunks = frames.chunks(pieces, B)
+            first = next(chunks, None)
+            if first is None:
+                steps = iter(())
+            else:
+                fp = FusedPass(model, tuple(first[0].shape[1:3]), B, total_frames=None, median=median)
+                # after the last chunk, the pass's final entry (the ball's tail) covers no new frame
+                steps = ((sizes.popleft() if sizes else 0, out)
+                         for out in fp.run(sized(itertools.chain([first], chunks))))
+        else:
+            steps = ((p.shape[0], {}) for p in pieces)
+        total, xyv = 0, {}
+        for n, out in steps:
+            for name in self.trackers:
+                if name == ball_name:
+                    for f, (x, y, v) in out.get(name, {}).items():
+                        xyv[f] = (x, y, v)
+                        merge.put(name, f, Ball(frame=f, xy=(x, y), visibility=v))
+                elif name in fixed:
+                    for f in range(total, total + n):
+                        merge.put(name, f, fixed[name])
+                else:
+                    for i, o in enumerate(out.get(name, [])):
+                        merge.put(name, total + i, o)
+            total += n
+            yield from self._emit(merge)
+        if ball is not None:  # TrackNet gives no frame of a stream shorter than a window: no ball there
+            for f in range(merge.next[ball_name], total):
+                merge.put(ball_name, f, Ball(frame=f, xy=(0.0, 0.0), visibility=0))
+        yield from self._emit(merge)
+        if ball is not None:
+            ball.results.predictions = ball.balls(xyv, total)  # InpaintNet over the whole trajectory
+        for t in self.trackers.values():  # what run() does after its pass
+            if t.stage in ("detect", "ball"):
+                t.to("cpu")
+            t.save_predictions()
+
+    def _emit(self, merge: FrameMerge) -> Iterator[tuple[int, dict]]:
+        for f, entry in merge.ready():
+            for name, obj in entry.items():
+                self.trackers[name].results.predictions.append(obj)
+            yield f, entry
 
     # ---- drawing pass (runner.py:91-173) -----------------------------------------------------------------------
     def _as_clip(self, frame_source) -> tuple[list, list, list]:
