@@ -192,6 +192,11 @@ int pb_u8_to_f16_nhwc16(const uint8_t* src, int B, int H, int W, void* dst, int 
  * may come from several clips, each with its own median.                                                          */
 int pb_tracknet_pack_windows_rows(const void* frames, int ring, const int* row_slot, const void* medians,
                                   const int* row_median, int B, int H, int W, void* x, void* stream);
+/* The same x, with each row's frames named by a table: row b = [medians[row_median[b]](3), frames[slots[b*8+0]](3) ...
+ * frames[slots[b*8+7]](3), 0 x5].  slots: int (B,8), row_median: int (B), on the device.  A row's 8 frames may sit
+ * anywhere in the pool (several interleaved streams sharing one pool of slots).                                  */
+int pb_tracknet_pack_windows_slots(const void* frames, const int* slots, const void* medians, const int* row_median,
+                                   int B, int H, int W, void* x, void* stream);
 
 /* ---- YOLOv8 head decode + NMS (ultralytics Detect/Pose decode, ops.non_max_suppression; SURVEY App. A.3-A.4) --- */
 typedef struct pb_yolo_level {
@@ -271,6 +276,19 @@ int pb_median_u8(const uint8_t* frames, int T, long long frame_bytes, uint8_t* o
  * that every window a frame needs is in pred.                                                                     */
 int pb_tracknet_ensemble_rows(const float* pred, int first_window, const int* desc, int nframes, int H, int W,
                               float thr, uint8_t* mask, float* ens, void* stream);
+/* Temporal ensemble + >thr with each frame's windows named by a table (several interleaved streams, each with its own
+ * carried windows).  carry: float (carry_rows,8,H,W); fresh: float (nb,8,H,W), this batch's windows.  table: int
+ * (nframes,9) on the device, per output frame: ref[k], k = 0..7, the row of window n-7+k of the frame's stream (its
+ * channel 7-k is read): carry row ref if ref < carry_rows, fresh row ref - carry_rows otherwise, -1 if absent; then
+ * the rule: 0 = weighted sum of the 8 windows, d > 0 = sum of the windows present / d (head, tail).  Rule 0 expects
+ * all 8 windows present; a -1 under rule 0 adds nothing (no out-of-bounds read), which is not an ensemble of any
+ * frame.  The arithmetic equals pb_tracknet_ensemble_rows' term for term.  mask, ens as there.                    */
+int pb_tracknet_ensemble_table(const float* carry, int carry_rows, const float* fresh, const int* table, int nframes,
+                               int H, int W, float thr, uint8_t* mask, float* ens, void* stream);
+/* carry[copies[2c]] = fresh[copies[2c+1]] for c < ncopies: whole (8,H,W) float heat-map rows.  copies: int
+ * (ncopies,2) on the device; no two copies share a destination.                                                   */
+int pb_tracknet_carry_rows(float* carry, const float* fresh, const int* copies, int ncopies, int H, int W,
+                           void* stream);
 /* 8-connected components of each mask; picks the component with max bbox area (ties: the one whose first pixel in
  * raster order comes last, = cv2.findContours order + predict_location's strict '>' scan).
  * bbox: int (nframes,4) = x,y,w,h (0,0,0,0 if empty). scratch: int32 (nframes, 5, H*W).                          */

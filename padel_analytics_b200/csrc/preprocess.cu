@@ -268,6 +268,31 @@ __global__ void u8_to_f16_nhwc16_kernel(const uint8_t* __restrict__ src, long np
   }
 }
 
+// One packed pixel of a TrackNet window: [median(3), frame 0(3), ..., frame 7(3), 0*5] as 32 fp16 values (64 bytes).
+__device__ __forceinline__ void store_window_pixel(uint4* __restrict__ o, uint2 m, const uint2 (&p)[8]) {
+  unsigned short h[32];
+  h[0] = (unsigned short)(m.x & 0xFFFF);
+  h[1] = (unsigned short)(m.x >> 16);
+  h[2] = (unsigned short)(m.y & 0xFFFF);
+#pragma unroll
+  for (int f = 0; f < 8; ++f) {
+    h[3 + 3 * f] = (unsigned short)(p[f].x & 0xFFFF);
+    h[4 + 3 * f] = (unsigned short)(p[f].x >> 16);
+    h[5 + 3 * f] = (unsigned short)(p[f].y & 0xFFFF);
+  }
+#pragma unroll
+  for (int j = 27; j < 32; ++j) h[j] = 0;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    uint4 v;
+    v.x = (uint32_t)h[8 * q + 0] | ((uint32_t)h[8 * q + 1] << 16);
+    v.y = (uint32_t)h[8 * q + 2] | ((uint32_t)h[8 * q + 3] << 16);
+    v.z = (uint32_t)h[8 * q + 4] | ((uint32_t)h[8 * q + 5] << 16);
+    v.w = (uint32_t)h[8 * q + 6] | ((uint32_t)h[8 * q + 7] << 16);
+    o[q] = v;
+  }
+}
+
 // x[b, h, w, :] = [median(3), frame[slot+0](3), ..., frame[slot+7](3), 0*5]   (32 channels, fp16), where row b's
 // frames are the ring slots (row_slot[b] + f) % ring and its median is medians[row_median[b]]: a batch of windows may
 // span several clips (each clip has its own median, and the ring skips the 7 frames at the end of a clip that start no
@@ -281,33 +306,29 @@ __global__ void tracknet_pack_rows_kernel(const uint2* __restrict__ frames, int 
     const int pix = (int)(i % HW);
     const int b = (int)(i / HW);
     const int first_slot = __ldg(row_slot + b);
-    unsigned short h[32];
-    {
-      const uint2 m = __ldg(medians + (size_t)__ldg(row_median + b) * HW + pix);
-      h[0] = (unsigned short)(m.x & 0xFFFF);
-      h[1] = (unsigned short)(m.x >> 16);
-      h[2] = (unsigned short)(m.y & 0xFFFF);
-    }
+    const uint2 m = __ldg(medians + (size_t)__ldg(row_median + b) * HW + pix);
+    uint2 p[8];
 #pragma unroll
-    for (int f = 0; f < 8; ++f) {
-      const int slot = (first_slot + f) % ring;
-      const uint2 p = __ldg(frames + (size_t)slot * HW + pix);
-      h[3 + 3 * f] = (unsigned short)(p.x & 0xFFFF);
-      h[4 + 3 * f] = (unsigned short)(p.x >> 16);
-      h[5 + 3 * f] = (unsigned short)(p.y & 0xFFFF);
-    }
+    for (int f = 0; f < 8; ++f) p[f] = __ldg(frames + (size_t)((first_slot + f) % ring) * HW + pix);
+    store_window_pixel(x + i * 4, m, p);
+  }
+}
+
+// The same window rows with each row's 8 frames named by a table: row b reads pool slots slots[b * 8 + f], f = 0..7,
+// and median medians[row_median[b]].  The frames of one row need not be contiguous or in any order in the pool, so a
+// batch may hold windows of several interleaved live streams whose frames share one slot pool.
+__global__ void tracknet_pack_slots_kernel(const uint2* __restrict__ frames, const int* __restrict__ slots,
+                                           const uint2* __restrict__ medians, const int* __restrict__ row_median,
+                                           int B, int HW, uint4* __restrict__ x) {
+  const long total = (long)B * HW;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int pix = (int)(i % HW);
+    const int b = (int)(i / HW);
+    const uint2 m = __ldg(medians + (size_t)__ldg(row_median + b) * HW + pix);
+    uint2 p[8];
 #pragma unroll
-    for (int j = 27; j < 32; ++j) h[j] = 0;
-    uint4* o = x + i * 4;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      uint4 v;
-      v.x = (uint32_t)h[8 * q + 0] | ((uint32_t)h[8 * q + 1] << 16);
-      v.y = (uint32_t)h[8 * q + 2] | ((uint32_t)h[8 * q + 3] << 16);
-      v.z = (uint32_t)h[8 * q + 4] | ((uint32_t)h[8 * q + 5] << 16);
-      v.w = (uint32_t)h[8 * q + 6] | ((uint32_t)h[8 * q + 7] << 16);
-      o[q] = v;
-    }
+    for (int f = 0; f < 8; ++f) p[f] = __ldg(frames + (size_t)__ldg(slots + b * 8 + f) * HW + pix);
+    store_window_pixel(x + i * 4, m, p);
   }
 }
 
@@ -402,6 +423,19 @@ int pb_tracknet_pack_windows_rows(const void* frames, int ring, const int* row_s
   tracknet_pack_rows_kernel<<<grid_for(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const uint2*>(frames), ring, row_slot, reinterpret_cast<const uint2*>(medians), row_median, B,
       H * W, reinterpret_cast<uint4*>(x));
+  PB_CUDA(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+int pb_tracknet_pack_windows_slots(const void* frames, const int* slots, const void* medians, const int* row_median,
+                                   int B, int H, int W, void* x, void* stream) {
+  PB_CHECK(frames && slots && medians && row_median && x, "tracknet_pack_slots: null pointer");
+  if (B <= 0) return 0;
+  const long total = (long)B * H * W;
+  tracknet_pack_slots_kernel<<<grid_for(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<const uint2*>(frames), slots, reinterpret_cast<const uint2*>(medians), row_median, B, H * W,
+      reinterpret_cast<uint4*>(x));
   PB_CUDA(cudaGetLastError());
   count_launch();
   return 0;

@@ -47,6 +47,60 @@ __global__ void ensemble_rows_kernel(const float* __restrict__ pred, int first_w
   }
 }
 
+// The ensemble of frames whose windows are named by a table: the frames may belong to several interleaved live
+// streams, each with its own carried windows.  table[f] = (ref[0..7], rule): ref[k] is the heat-map row of window
+// n-7+k of frame f's stream (its channel 7-k is read): a row of the carry pool when < carry_rows, row ref - carry_rows
+// of this batch's fresh rows otherwise, or -1 when the window does not exist.  rule 0: the weighted sum of the 8
+// windows; rule d > 0: the head/tail mean, the sum of the windows present divided by d.  The arithmetic is that of
+// ensemble_rows_kernel term for term, so a stream's masks are bit-identical to the single-stream path.
+__global__ void ensemble_table_kernel(const float* __restrict__ carry, int carry_rows, const float* __restrict__ fresh,
+                                      const int* __restrict__ table, int nframes, int HW, float thr,
+                                      uint8_t* __restrict__ mask, float* __restrict__ ens) {
+  const long total = (long)nframes * HW;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int pix = (int)(i % HW);
+    const int* t = table + (i / HW) * 9;
+    const int rule = __ldg(t + 8);
+    float acc = 0.f;
+    float result;
+    if (rule == 0) {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const float wk = (float)(k < 4 ? k + 1 : 8 - k) / 20.0f;
+        const int r = __ldg(t + k);
+        if (r < 0) continue;  // never planned: an absent window adds nothing rather than reading out of bounds
+        const float* row = r < carry_rows ? carry + (size_t)r * 8 * HW : fresh + (size_t)(r - carry_rows) * 8 * HW;
+        acc = __fadd_rn(acc, __fmul_rn(row[(size_t)(7 - k) * HW + pix], wk));  // mul, then add (no FMA)
+      }
+      result = acc;
+    } else {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const int r = __ldg(t + k);
+        if (r >= 0) {
+          const float* row = r < carry_rows ? carry + (size_t)r * 8 * HW : fresh + (size_t)(r - carry_rows) * 8 * HW;
+          acc += row[(size_t)(7 - k) * HW + pix];
+        }
+      }
+      result = acc / (float)rule;
+    }
+    mask[i] = result > thr ? 1 : 0;
+    if (ens) ens[i] = result;
+  }
+}
+
+// carry[copies[2c]] = fresh[copies[2c + 1]]: whole (8, H, W) heat-map rows, 16 bytes per thread.
+__global__ void carry_rows_kernel(float4* __restrict__ carry, const float4* __restrict__ fresh,
+                                  const int* __restrict__ copies, int ncopies, long row_vec) {
+  const long total = (long)ncopies * row_vec;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int c = (int)(i / row_vec);
+    const long e = i % row_vec;
+    const size_t dst = (size_t)__ldg(copies + 2 * c) * row_vec, src = (size_t)__ldg(copies + 2 * c + 1) * row_vec;
+    carry[dst + e] = __ldcs(fresh + src + e);
+  }
+}
+
 __device__ __forceinline__ int uf_find(const int* parent, int i) {
   int p = __ldcg(parent + i);
   while (p != i) {
@@ -179,6 +233,38 @@ int pb_tracknet_ensemble_rows(const float* pred, int first_window, const int* de
   if (blocks > (long)num_sms() * 32) blocks = (long)num_sms() * 32;
   ensemble_rows_kernel<<<(int)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       pred, first_window, desc, nframes, H * W, thr, mask, ens);
+  PB_CUDA(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+int pb_tracknet_ensemble_table(const float* carry, int carry_rows, const float* fresh, const int* table, int nframes,
+                               int H, int W, float thr, uint8_t* mask, float* ens, void* stream) {
+  PB_CHECK(carry && fresh && table && mask, "ensemble_table: null pointer");
+  PB_CHECK((reinterpret_cast<uintptr_t>(table) & 3) == 0, "ensemble_table: table must be 4-byte aligned");
+  if (nframes <= 0) return 0;
+  const long total = (long)nframes * H * W;
+  long blocks = (total + 255) / 256;
+  if (blocks > (long)num_sms() * 32) blocks = (long)num_sms() * 32;
+  ensemble_table_kernel<<<(int)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      carry, carry_rows, fresh, table, nframes, H * W, thr, mask, ens);
+  PB_CUDA(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+int pb_tracknet_carry_rows(float* carry, const float* fresh, const int* copies, int ncopies, int H, int W,
+                           void* stream) {
+  PB_CHECK(carry && fresh && copies, "carry_rows: null pointer");
+  PB_CHECK(((reinterpret_cast<uintptr_t>(carry) | reinterpret_cast<uintptr_t>(fresh)) & 15) == 0,
+           "carry_rows: carry and fresh must be 16-byte aligned");
+  if (ncopies <= 0) return 0;
+  const long row_vec = (long)8 * H * W / 4;
+  const long total = (long)ncopies * row_vec;
+  long blocks = (total + 255) / 256;
+  if (blocks > (long)num_sms() * 32) blocks = (long)num_sms() * 32;
+  carry_rows_kernel<<<(int)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<float4*>(carry), reinterpret_cast<const float4*>(fresh), copies, ncopies, row_vec);
   PB_CUDA(cudaGetLastError());
   count_launch();
   return 0;

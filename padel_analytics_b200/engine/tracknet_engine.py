@@ -218,9 +218,11 @@ class BallPipeline:
         self.set_median(median_rgb)
         self.reset()
 
-    def _init_buffers(self, engine: TrackNetEngine, frame_hw, ring: int, pool: int, max_frames: int):
+    def _init_buffers(self, engine: TrackNetEngine, frame_hw, ring: int, pool: int, max_frames: int,
+                      table_ints: int | None = None):
         """Pillow bicubic tables (frame size -> network size), the ring of `ring` resized frames, a pool of `pool`
-        backgrounds, and the per-batch buffers for up to `max_frames` emitted frames."""
+        backgrounds, and the per-batch buffers for up to `max_frames` emitted frames and `table_ints` table entries
+        (default: the row tables of `_launch_batch`)."""
         self.eng = engine
         self.dev = engine.device
         self.Hs, self.Ws = frame_hw
@@ -238,7 +240,8 @@ class BallPipeline:
         self.scratch = torch.zeros((B + 7, 5, H * W), dtype=torch.int32, device=self.dev)  # boxes run B+7 at a time
         self.bbox = torch.zeros((max_frames, 4), dtype=torch.int32, device=self.dev)
         # a batch's tables on the device: row ring slots (B), row median slots (B), frame descriptors (max_frames, 3)
-        self._tables = torch.zeros(2 * B + 3 * max_frames, dtype=torch.int32, device=self.dev)
+        self._tables = torch.zeros(2 * B + 3 * max_frames if table_ints is None else table_ints, dtype=torch.int32,
+                                   device=self.dev)
         # per launch slot, pinned: the staged tables and the downloaded boxes (see _launch_batch for the slot rule)
         self._stage = [torch.zeros(self._tables.shape, dtype=torch.int32).pin_memory() for _ in range(4)]
         self._host_ring = [torch.zeros((max_frames, 4), dtype=torch.int32).pin_memory() for _ in range(4)]
@@ -258,6 +261,11 @@ class BallPipeline:
         self._median_src = med.cpu().clone()
         dev_med = med.to(self.dev).contiguous().view(1, self.Hs, self.Ws, 3)
         self._resize(dev_med, 1, self.medians[:1], swap_rb=0)
+
+    def load_median(self, slot: int, median_rgb) -> None:
+        """(Hs,Ws,3) uint8 RGB background (host or device) -> resized into pool slot `slot`, as `set_median` does."""
+        med = torch.as_tensor(median_rgb).to(self.dev, torch.uint8).contiguous().view(1, self.Hs, self.Ws, 3)
+        self._resize(med, 1, self.medians[slot:slot + 1], swap_rb=0)
 
     def reset(self, base: int = 0):
         """base = absolute index of the first frame that will be pushed (= first window computed); > 0 for shards
@@ -359,12 +367,7 @@ class BallPipeline:
             i = bad[0]
             raise L.PbError(f"ensemble: frame {desc[i, 2]} needs windows [{lo[i]},{hi[i]}], the buffer holds "
                             f"[{first_window - 7},{first_window + nb})")
-        # The slot's staged tables and host boxes are rewritten only once its previous launch has completed.  That
-        # launch was waited for at the end of the launch before this one, unless that launch raised midway.
-        slot = self._turn
-        self._turn = (slot + 1) % len(self._pending)
-        if self._pending[slot] is not None:
-            self._pending[slot]()
+        slot = self._claim_slot()
         stage = self._stage[slot]
         n = 2 * nb + 3 * nframes
         t = stage.numpy()
@@ -382,15 +385,33 @@ class BallPipeline:
             ens_ptr = self.ens.data_ptr()
         L.check(L.lib().pb_tracknet_ensemble_rows(eng.pred.data_ptr(), first_window - 7, rows + 8 * nb, nframes, eng.H,
                                                   eng.W, 0.5, self.mask.data_ptr(), ens_ptr, L.stream_ptr()))
-        step = self.scratch.shape[0]
-        for f in range(0, nframes, step):  # the scratch holds B+7 frames: several launches for the short-clip case
-            m = min(step, nframes - f)
-            L.check(L.lib().pb_ccl_bbox(self.mask[f:].data_ptr(), m, eng.H, eng.W, self.scratch.data_ptr(),
-                                        self.bbox[f:].data_ptr(), L.stream_ptr()))
+        self._boxes(nframes)
         # carry the last 7 windows for the next batch (ball_tracker.py:523), which may start another clip
         if nb:
             carry = eng.pred[nb:nb + 7].clone()
             eng.pred[:7].copy_(carry)
+        return self._download(slot, key, nframes)
+
+    def _claim_slot(self) -> int:
+        """The next launch slot.  The slot's staged tables and host boxes are rewritten only once its previous launch
+        has completed.  That launch was waited for at the end of the launch before this one, unless that launch raised
+        midway."""
+        slot = self._turn
+        self._turn = (slot + 1) % len(self._pending)
+        if self._pending[slot] is not None:
+            self._pending[slot]()
+        return slot
+
+    def _boxes(self, nframes: int) -> None:
+        """Boxes of the first `nframes` masks."""
+        step = self.scratch.shape[0]
+        for f in range(0, nframes, step):  # the scratch holds B+7 frames: several launches for the short-clip case
+            m = min(step, nframes - f)
+            L.check(L.lib().pb_ccl_bbox(self.mask[f:].data_ptr(), m, self.eng.H, self.eng.W, self.scratch.data_ptr(),
+                                        self.bbox[f:].data_ptr(), L.stream_ptr()))
+
+    def _download(self, slot: int, key, nframes: int):
+        """Enqueue the download of the first `nframes` boxes into launch slot `slot`; returns the launch's finish."""
         host = self._host_ring[slot]
         host[:nframes].copy_(self.bbox[:nframes], non_blocking=True)
         done = torch.cuda.Event()
@@ -433,11 +454,6 @@ class ClipBallPipeline(BallPipeline):
             raise L.PbError("ClipBallPipeline: the plan was made for another ring, pool or batch size")
         self.eng.pred.zero_()
 
-    def load_median(self, slot: int, median_rgb: torch.Tensor) -> None:
-        """(Hs,Ws,3) uint8 RGB background (device) -> resized into pool slot `slot`, as BallPipeline.set_median does."""
-        med = median_rgb.to(self.dev, torch.uint8).contiguous().view(1, self.Hs, self.Ws, 3)
-        self._resize(med, 1, self.medians[slot:slot + 1], swap_rb=0)
-
     def push_at(self, frames_bgr: torch.Tensor, slot: int) -> None:
         """Resize (n,Hs,Ws,3) uint8 BGR device frames into ring slots slot..slot+n-1."""
         n = frames_bgr.shape[0]
@@ -450,6 +466,78 @@ class ClipBallPipeline(BallPipeline):
         """Enqueue one planned batch; returns a callable that waits and yields (frames [(clip, frame)], host int32
         (nframes, 4) boxes)."""
         return self._launch_batch(batch.frames, batch.first_window, batch.row_slot, batch.row_median, batch.desc)
+
+
+class StreamsBallPipeline(BallPipeline):
+    """BallPipeline over several interleaved live streams in one pass: a device batch may hold windows of any open
+    streams, each at its own position.  The host planner (`stream_plan.StreamPlanner`) places each pushed frame in a
+    shared pool of resized frames, gives each stream a lane (7 rows of a heat-map carry pool and a median pool slot)
+    and names, per launch, each row's 8 frame slots and each emitted frame's 8 heat-map rows.  Per stream the boxes
+    are bit-identical to BallPipeline run on that stream alone."""
+
+    def __init__(self, engine: TrackNetEngine, frame_hw: tuple[int, int], max_open: int):
+        from .stream_plan import StreamPlanner
+
+        plan = StreamPlanner(engine.B, max_open)
+        B, F = engine.B, plan.max_frames
+        # tables of a launch: row slots (B, 8), row medians (B), frame refs + rule (F, 9), carry copies (B, 2)
+        self._init_buffers(engine, frame_hw, ring=plan.n_slots, pool=max_open, max_frames=F,
+                           table_ints=9 * B + 9 * F + 2 * B)
+        self.max_open = max_open
+        self.carry = torch.zeros((plan.carry_rows, 8, engine.H, engine.W), dtype=torch.float32, device=self.dev)
+        self.begin()
+
+    def begin(self) -> None:
+        """Start a pass: no stream open, every slot free."""
+        from .stream_plan import StreamPlanner
+
+        self.plan = StreamPlanner(self.B, self.max_open)
+
+    def step_async(self, frames_bgr: torch.Tensor, segments: list, ends: list, median_of):
+        """One upload chunk: (n,Hs,Ws,3) uint8 BGR device frames made of `segments` = [(key, frames)] runs of one
+        stream each, after which the streams `ends` end.  Loads the backgrounds of the streams that start
+        (`median_of(key)`: (Hs,Ws,3) uint8 RGB), resizes the frames into their pool slots and enqueues the step's
+        launches.  Returns (the planned `StreamStep`, the launches' finish callables, each yielding ([(key, frame)],
+        host int32 (nframes, 4) boxes))."""
+        st = self.plan.step(segments, ends)
+        for key, lane in st.medians:
+            self.load_median(lane, median_of(key))
+        for off, n, slot in st.pushes:
+            self._resize(frames_bgr[off:off + n].contiguous(), n, self.small[slot:slot + n], swap_rb=1)
+        return st, [self._launch_table(launch) for launch in st.launches]
+
+    def _launch_table(self, launch):
+        """Enqueue one planned launch (`stream_plan.StreamLaunch`): pack, TrackNet, ensemble + threshold, carry
+        update, boxes, download."""
+        eng = self.eng
+        nb, nf, nc = len(launch.rows), len(launch.frames), len(launch.carry)
+        slot = self._claim_slot()
+        t = self._stage[slot].numpy()
+        a, b = 8 * nb, 9 * nb
+        c = b + 9 * nf
+        d = c + 2 * nc
+        if nb:
+            t[:a] = np.asarray(launch.row_slots).reshape(-1)
+            t[a:b] = launch.row_median
+        if nf:
+            t[b:c] = np.concatenate([np.asarray(launch.refs), np.asarray(launch.rule)[:, None]], 1).reshape(-1)
+        if nc:
+            t[c:d] = np.asarray(launch.carry).reshape(-1)
+        self._tables[:d].copy_(self._stage[slot][:d], non_blocking=True)
+        p = self._tables.data_ptr()
+        fresh = eng.pred[7:]
+        if nb:  # nb = 0: tails ensembled from the carry pool alone
+            L.check(L.lib().pb_tracknet_pack_windows_slots(self.small.data_ptr(), p, self.medians.data_ptr(), p + 4 * a,
+                                                           nb, eng.H, eng.W, eng.x.data_ptr(), L.stream_ptr()))
+            eng.run_packed()
+        L.check(L.lib().pb_tracknet_ensemble_table(self.carry.data_ptr(), self.carry.shape[0], fresh.data_ptr(),
+                                                   p + 4 * b, nf, eng.H, eng.W, 0.5, self.mask.data_ptr(), None,
+                                                   L.stream_ptr()))
+        # after the ensemble: window w's carry row is window w-7's, which frame w reads
+        L.check(L.lib().pb_tracknet_carry_rows(self.carry.data_ptr(), fresh.data_ptr(), p + 4 * c, nc, eng.H, eng.W,
+                                               L.stream_ptr()))
+        self._boxes(nf)
+        return self._download(slot, launch.frames, nf)
 
 
 def bbox_to_xyv(bbox: np.ndarray, img_scaler: tuple[float, float]):

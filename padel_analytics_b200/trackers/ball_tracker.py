@@ -22,7 +22,7 @@ import numpy as np
 import torch
 
 from ..engine.inpaint_engine import InpaintNetEngine
-from ..engine.tracknet_engine import BallPipeline, ClipBallPipeline, TrackNetEngine, bbox_to_xyv
+from ..engine.tracknet_engine import BallPipeline, ClipBallPipeline, StreamsBallPipeline, TrackNetEngine, bbox_to_xyv
 from .tracker import NoPredictSample, Object, Tracker
 
 
@@ -122,6 +122,7 @@ class BallTracker(Tracker):
         self.median = median
         self._pipe = None
         self._clip_pipe = None
+        self._streams_pipe = None
 
     def video_info_post_init(self, video_info) -> "BallTracker":
         self.video_info = video_info
@@ -229,6 +230,26 @@ class BallTracker(Tracker):
             self._clip_pipe = ClipBallPipeline(self.tracknet, tuple(frame_hw))
         return self._clip_pipe
 
+    def streams_begin(self, frame_hw, max_open: int, steps, median_of):
+        """Streaming over several interleaved live streams (`TrackingRunner.stream_many`): `steps` is a deque to which
+        the caller appends, before each `stream_push_async`, the chunk's ([(key, frames)] runs, [keys ending]);
+        `median_of(key)` returns the stream's (H,W,3) uint8 RGB background.  Each push's finish then yields
+        [(key, frame, (x, y, vis))].  Ball coordinates are scaled by `video_info`, shared by every stream."""
+        pipe = self._streams_pipe
+        if pipe is None or (pipe.Hs, pipe.Ws) != tuple(frame_hw) or pipe.max_open != max_open:
+            pipe = self._streams_pipe = StreamsBallPipeline(self.tracknet, tuple(frame_hw), max_open)
+        pipe.begin()
+        self._stream = dict(streams=steps, median_of=median_of,
+                            scaler=(self.video_info.width / self.WIDTH, self.video_info.height / self.HEIGHT))
+        return pipe
+
+    def _streams_push_async(self, frames: torch.Tensor):
+        s = self._stream
+        segments, ends = s["streams"].popleft()
+        _, fins = self._streams_pipe.step_async(frames, segments, ends, s["median_of"])
+        fin = self._xyv_finish(fins, lambda frames: frames)  # a launch yields its [(key, frame)]
+        return lambda: [(k, f, v) for (k, f), v in fin()]
+
     def _xyv_finish(self, fins, frames_of):
         """A callable that waits for the launches `fins` in turn and returns [(frame, (x, y, vis))] for their boxes;
         frames_of(key) gives the frames of the launch that yields (key, boxes)."""
@@ -267,6 +288,8 @@ class BallTracker(Tracker):
         window that became computable; returns a callable that waits and yields {frame: (x, y, vis)}."""
         if "clips" in self._stream:
             return self._clips_push_async(frames)
+        if "streams" in self._stream:
+            return self._streams_push_async(frames)
         pipe, s = self._pipe, self._stream
         pipe.push_frames(frames)
         fin = self._xyv_finish(pipe.run_ready_async(s["total"]), itertools.count)  # a launch yields its first frame

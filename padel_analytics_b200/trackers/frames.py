@@ -63,9 +63,15 @@ def chunks(pieces: Iterable[torch.Tensor], B: int, alloc: Callable[[tuple], torc
     and device pieces pass through as slices; host frames that are not pinned are gathered into three (B,H,W,3)
     buffers from `alloc(shape)`, allocated on first need and refilled in turn: a chunk's buffer is refilled three
     chunks later, which a consumer with one chunk of look-ahead (`FusedPass.run`, `OverlayRenderer.run`) has uploaded
-    by then."""
+    by then.  A piece that is None closes the chunk being filled: it is yielded at once, short or even empty."""
     bufs, out, n, k, run0 = [], [], 0, 0, None  # run0: where the gathered run of the current chunk starts
     for t in pieces:
+        if t is None:
+            if run0 is not None:
+                out.append(bufs[k % 3][run0:n])
+            yield out
+            out, n, k, run0 = [], 0, k + 1, None
+            continue
         while t.shape[0]:
             take = min(B - n, t.shape[0])
             part, t = t[:take], t[take:]

@@ -70,6 +70,12 @@ def ball_shard_frames(total: int, start: int, end: int) -> tuple[int, int]:
     return max(0, start - 7), min(total, end + 7)
 
 
+def _host_state(t: Tracker) -> dict:
+    """A tracker's order-dependent host state, as `video_info_post_init` sets it (PlayerTracker: its ByteTrack); put
+    back with `t.__dict__.update(state)`."""
+    return {k: t.__dict__[k] for k in ("video_info", "byte_track") if k in t.__dict__}
+
+
 def _batch_trackers(trackers: dict[str, Tracker]) -> dict[str, Tracker]:
     """The trackers a device pass (`FusedPass`, `ClipPass`) feeds: those of stage "detect" or "ball"."""
     return {n: t for n, t in trackers.items() if t.stage in ("detect", "ball")}
@@ -278,6 +284,192 @@ class ClipPass(FusedPass):
         return out
 
 
+class StreamsPass(FusedPass):
+    """FusedPass over the frames of several interleaved live streams (`TrackingRunner.stream_many`).  Upload chunk i
+    holds the frames `StreamMux` put in it, runs of consecutive frames of one stream each, and may be short or empty
+    when a stream ends (its tail is then not held back by frames still to come).  The YOLO engines see one batch of
+    frames; their host post-processing runs once per run, in pull order, with that stream's own host state
+    (`_host_state`: PlayerTracker gets a fresh ByteTrack at the stream's first frame).  The ball tracker runs its
+    windows through the multi-stream planner (`BallTracker.streams_begin`).  Per chunk, `run` yields ((runs
+    [(key, first frame, n)], ending keys), {tracker name: results}): [(key, first frame, objects)] for the YOLO
+    trackers, [(key, frame, (x, y, vis))] for the ball tracker."""
+
+    def __init__(self, trackers: dict[str, Tracker], frame_hw: tuple[int, int], batch_size: int, max_open: int,
+                 metas: collections.deque, median_of: Callable, video_info, streams: Optional[int] = None):
+        self.metas = metas  # (runs, ends) per chunk, appended by StreamMux before the chunk is handed over
+        self.max_open = max_open
+        self.median_of = median_of
+        self.video_info = video_info
+        self.host: dict = {}  # stream key -> {tracker name: host state}
+        self._ball_steps = collections.deque()
+        super().__init__(trackers, frame_hw, batch_size, total_frames=None, streams=streams)
+
+    def _begin_ball(self, total_frames, first_frame, emit_range, median) -> None:
+        for t in self.trackers.values():
+            if t.stage == "ball":
+                t.streams_begin(self.hw, self.max_open, self._ball_steps, self.median_of)
+
+    def _launch(self, fr: torch.Tensor):
+        meta = self.metas.popleft()
+        runs, ends = meta
+        balls = {n: t for n, t in self.trackers.items() if t.stage == "ball"}
+        if balls:
+            self._ball_steps.append(([(key, n) for key, _, n in runs], ends))
+        if fr.shape[0]:
+            pending, _ = super()._launch(fr)
+        else:  # a stream ended at a chunk boundary: its tail alone
+            pending = [(name, t, t.stream_push_async(fr)) for name, t in balls.items()]
+        return pending, meta
+
+    def _finish(self, launched):
+        pending, meta = launched
+        runs, ends = meta
+        out = {}
+        for name, t, fin in pending:
+            res = fin()
+            if t.stage == "ball":
+                out[name] = res
+                continue
+            parts, a = [], 0
+            for key, f0, n in runs:
+                if f0 == 0:
+                    t.video_info_post_init(self.video_info)
+                else:
+                    t.__dict__.update(self.host[key][name])
+                parts.append((key, f0, t.postprocess(res[a:a + n], self.hw)))
+                self.host.setdefault(key, {})[name] = _host_state(t)
+                a += n
+            out[name] = parts
+        for key in ends:
+            self.host.pop(key, None)
+        return meta, out
+
+    def _end(self, total: int):
+        return None  # every stream ended in a chunk of its own
+
+
+class StreamMux:
+    """The (key, frames) items of `TrackingRunner.stream_many` as the pieces of one pass, in pull order: `pieces()`
+    yields (n,H,W,3) tensors and None, which closes the upload chunk being filled (`frames.chunks`), and appends to
+    `metas`, before handing over the piece that completes it, each chunk's (runs [(key, first frame, n)], keys
+    ending after its frames).
+
+    A chunk closes when it holds B frames, when B frames have been pulled since the chunk before it closed (frames
+    held for a background count: they are pulled but enter no chunk yet), and at a stream's end, whichever comes
+    first.  So a chunk never waits longer than B pulls, however many streams are held, and a stream's tail is not held
+    back by frames of other streams still to come.  A chunk may be short, or empty.
+
+    A stream without a background (`medians[key]`, else `default`) has its first `hold` frames copied to the device
+    and held; its frames enter the pass when `background(pieces)` has been taken from them (or at its end, from the
+    frames it has), and until then the other streams keep running.  ValueError: a frame of another size than the
+    first stream's, a key that reappears after its end, more than `max_open` streams open at once."""
+
+    def __init__(self, items: Iterable, batch: int, max_open: int, medians: Optional[dict] = None, default=None,
+                 hold: int = 0, background: Optional[Callable] = None, hold_device: str = "cuda"):
+        self.items, self.B, self.max_open, self.hold_device = items, batch, max_open, hold_device
+        self.medians = dict(medians or {})
+        self.default, self.hold, self.background = default, hold, background
+        self.metas = collections.deque()
+        self.hw = None  # the frame size, fixed by the first frame
+        self.count: dict = {}  # per open stream: frames handed to the pass
+        self.held: dict = {}  # per open stream waiting for its background: the device copies of its first frames
+        self.ended: set = set()
+        # the chunk being filled: its runs, the streams ending after it, its frames, the frames pulled since it opened
+        self._runs, self._ends, self._n, self._pulls = [], [], 0, 0
+
+    def _put(self, key, t: torch.Tensor, pulled: bool) -> Iterator[Optional[torch.Tensor]]:
+        """Hand stream `key`'s frames t to the pass, split at chunk boundaries.  pulled: t was pulled just now, so
+        its frames also count toward the chunk's pulls (False for held frames released later)."""
+        f0 = self.count[key]
+        self.count[key] += t.shape[0]
+        while t.shape[0]:
+            take = min(self.B - (max(self._n, self._pulls) if pulled else self._n), t.shape[0])
+            self._runs.append((key, f0, take))
+            f0, self._n = f0 + take, self._n + take
+            self._pulls += take if pulled else 0
+            part, t = t[:take], t[take:]
+            if self._n == self.B:  # full: `frames.chunks` closes it on this piece
+                self._close()
+                yield part
+            elif self._pulls == self.B:
+                self._close()
+                yield part
+                yield None
+            else:
+                yield part
+
+    def _pull_held(self, n: int) -> Iterator[None]:
+        """n frames pulled into a hold: they enter no chunk, but count toward the chunk's pulls."""
+        while n:
+            take = min(self.B - self._pulls, n)
+            self._pulls, n = self._pulls + take, n - take
+            if self._pulls == self.B:
+                self._close()
+                yield None
+
+    def _close(self) -> None:
+        self.metas.append((self._runs, self._ends))
+        self._runs, self._ends, self._n, self._pulls = [], [], 0, 0
+
+    def _release(self, key) -> Iterator[Optional[torch.Tensor]]:
+        """Stream `key`'s held frames, now that its background exists (taken from them when it has any)."""
+        held = self.held.pop(key)
+        if held and self.background is not None:
+            self.medians[key] = self.background(held)
+        for t in held:
+            yield from self._put(key, t, pulled=False)
+
+    def _end(self, key) -> Iterator[Optional[torch.Tensor]]:
+        if key in self.held:
+            yield from self._release(key)
+        del self.count[key]
+        self.ended.add(key)
+        self._ends.append(key)
+
+    def pieces(self) -> Iterator[Optional[torch.Tensor]]:
+        for key, item in self.items:
+            if key in self.ended:
+                raise ValueError(f"stream_many: stream {key!r} appears again after its end")
+            if item is None:
+                if key not in self.count:  # a stream of no frame: nothing to track
+                    self.ended.add(key)
+                    self._ends.append(key)
+                    continue
+                yield from self._end(key)
+                self._close()
+                yield None
+                continue
+            t = next(frames.tensors([item], self.hw, f"stream {key!r}"))
+            self.hw = tuple(t.shape[1:3])
+            if key not in self.count:
+                if len(self.count) == self.max_open:
+                    raise ValueError(f"stream_many: stream {key!r} would be stream {self.max_open + 1} open at once, "
+                                     f"max_open is {self.max_open}")
+                self.count[key] = 0
+                if self.hold and key not in self.medians:
+                    if self.default is not None:
+                        self.medians[key] = self.default
+                    else:
+                        self.held[key] = []
+            if key in self.held:  # copied: the caller may reuse its buffer once the item is pulled
+                held = self.held[key]
+                room = self.hold - sum(p.shape[0] for p in held)
+                held.append(t[:room].to(self.hold_device, copy=True))
+                yield from self._pull_held(min(room, t.shape[0]))
+                if room > t.shape[0]:
+                    continue
+                yield from self._release(key)
+                t = t[room:]
+                if not t.shape[0]:
+                    continue
+            yield from self._put(key, t, pulled=True)
+        for key in list(self.count):
+            yield from self._end(key)
+        if self._runs or self._ends:
+            self._close()
+            yield None
+
+
 class FrameMerge:
     """In-order merge of per-tracker results for `TrackingRunner.stream`.  Each tracker's results arrive in frame
     order, but the trackers are out of step with one another: a YOLO tracker has a batch's frames when the batch is
@@ -334,6 +526,7 @@ class TrackingRunner:
         self._source = None  # frame_source of the last run(), for the drawing pass
         self._clip_reading: Optional[int] = None  # run_clips: the clip whose frames the pass read last
         self.timings: dict[str, float] = {}
+        self.stream_results: dict = {}  # stream_many: per ended stream, {tracker name: [Object per frame]}
 
     def restart(self) -> None:
         for t in self.trackers.values():
@@ -458,24 +651,30 @@ class TrackingRunner:
         look-ahead, the 7 frames the ball ensemble looks ahead), for every f whose frame f + 2B + 8 comes after the
         frames held for the background.  An item of n frames is pulled whole, which moves the bound by up to n - 1
         frames.  A live caller picks a small batch_size."""
+        self._check_streamable("stream")
+        return self._stream(frames_in, median)
+
+    def _check_streamable(self, what: str) -> None:
+        """ValueError for what a stream cannot run: a torch.distributed job, "frames" trackers, cached predictions, no
+        video_info."""
         import torch.distributed as dist
 
         if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
-            raise ValueError(f"stream: a stream runs in one process, not over a torch.distributed job of world size "
+            raise ValueError(f"{what}: a stream runs in one process, not over a torch.distributed job of world size "
                              f"{dist.get_world_size()}")
         if not self.trackers:
-            raise ValueError("stream: no trackers")
+            raise ValueError(f"{what}: no trackers")
         other = sorted(n for n, t in self.trackers.items() if t.stage not in ("detect", "ball", "fixed"))
         if other:
-            raise ValueError(f"stream: trackers {other} have no batch model stage (a YOLO or ball model) and no fixed "
+            raise ValueError(f"{what}: trackers {other} have no batch model stage (a YOLO or ball model) and no fixed "
                              "detection")
         cached = sorted(n for n, t in self.trackers.items() if len(t))
         if cached:
-            raise ValueError(f"stream: trackers {cached} hold cached predictions, and a stream has no frame count to "
+            raise ValueError(f"{what}: trackers {cached} hold cached predictions, and a stream has no frame count to "
                              "match them against (restart() them first)")
         if self.video_info is None:
-            raise ValueError("stream: the fps and the ball's frame size come from video_info, and this runner has none")
-        return self._stream(frames_in, median)
+            raise ValueError(f"{what}: the fps and the ball's frame size come from video_info, and this runner has "
+                             "none")
 
     def _stream(self, frames_in: Iterable, median) -> Iterator[tuple[int, dict]]:
         from .ball_tracker import median_background_device
@@ -553,6 +752,130 @@ class TrackingRunner:
                 self.trackers[name].results.predictions.append(obj)
             yield f, entry
 
+    # ---- several live streams in one pass ---------------------------------------------------------------------------
+    def stream_many(self, items: Iterable, medians: Optional[dict] = None, max_open: int = 16
+                    ) -> Iterator[tuple[object, int, dict]]:
+        """Track several live streams (cameras, courts) in one pass whose device batches hold frames of any of them: a
+        generator of `(key, frame index, {tracker name: Object})`, each stream's entries in frame order, each entry
+        yielded as soon as every tracker's result for it is final.  Each stream gets what `stream()` gives on its
+        frames alone.
+
+        items: any iterable of `(key, frames)`: `key` any hashable name of a stream, `frames` one HWC uint8 BGR frame
+        or a uint8 (n,H,W,3) batch, host or device, as `stream()` takes them.  `(key, None)` ends stream `key`; every
+        open stream ends when the iterable does.  Streams may open and end at any point; a key that ended may not
+        appear again (ValueError).  Every frame must have the size of the first (ValueError naming the key), and every
+        stream shares the runner's `video_info` (ByteTrack's fps, the ball's coordinate scale).  At most `max_open`
+        streams may be open at once (ValueError); the ball stage's device pools are sized for that many (about 42 MB
+        per open stream at TrackNet's 288x512, `StreamsBallPipeline`).
+
+        Refused with ValueError before any item is pulled: what `stream()` refuses ("frames" trackers, cached
+        predictions, a torch.distributed job of world size > 1, no `video_info`).
+
+        Per stream, the host stages run as if the stream ran alone: YOLO post-processing runs once per run of the
+        stream's frames in a batch, in pull order, with the stream's own ByteTrack (PlayerTracker: fresh at its first
+        frame).  The yielded Ball is TrackNet's.  When a stream ends, InpaintNet runs over its trajectory and
+        `stream_results[key]` = {tracker name: [Object per frame]} holds its final results, equal to `run()`'s on its
+        frames, before its last entries are yielded; the caller may pop them.  The trackers' own `results` are left
+        untouched and nothing is written to a `save_path`.
+
+        Background per stream: `medians[key]` ((H,W,3) uint8 RGB), else `BallTracker.median`, else the median of the
+        stream's first `median_max_sample_num` frames, which are held on the device until it is computed; until then
+        the stream's frames do not enter the pass and none of its entries is yielded, while the other streams run.
+
+        Latency: with B the pass's batch (the smallest batch_size of the "detect" and "ball" trackers), count the frames
+        of all streams in pull order, those held for a background included; if stream s's frame f + 7 is the k-th frame
+        pulled, the entry (s, f) is yielded before the (k + 2B)-th frame is pulled, for every f whose frame f + 7 is
+        pulled after s's background exists, whatever the other streams do.  A stream's last 7 entries are yielded
+        before the (B + 1)-th frame pulled after its end item.  Both hold because an upload chunk closes once B frames
+        have been pulled since the one before it closed, even when held frames left it short or empty, and at every
+        end item; the pass keeps one chunk of look-ahead.  An item of n frames is pulled whole, which moves the bounds
+        by up to n - 1 frames.
+
+        As `stream()`, this leaves Python's cyclic garbage collector as the caller set it."""
+        self._check_streamable("stream_many")
+        if max_open < 1:
+            raise ValueError("stream_many: max_open must be >= 1")
+        return self._stream_many(items, medians, max_open)
+
+    def _stream_many(self, items: Iterable, medians, max_open: int) -> Iterator[tuple[object, int, dict]]:
+        from .ball_tracker import median_background_device
+
+        model = _batch_trackers(self.trackers)
+        fixed = {n: t.fixed_detection for n, t in self.trackers.items() if t.stage == "fixed"}
+        ball_name, ball = next(((n, t) for n, t in model.items() if t.stage == "ball"), (None, None))
+        B = min(t.batch_size for t in model.values()) if model else 1
+        mux = StreamMux(items, B, max_open, medians, default=None if ball is None else ball.median,
+                        hold=0 if ball is None else ball.median_max_sample_num, background=median_background_device)
+        merges: dict = {}  # per stream: its FrameMerge
+        got: dict = {}  # per stream: {tracker name: objects yielded}
+        xyv: dict = {}  # per stream: its TrackNet trajectory
+        count: dict = {}  # per stream: frames seen
+
+        def step(meta, out) -> list:
+            runs, ends = meta
+            for key, f0, n in runs:
+                if key not in merges:
+                    merges[key], got[key], xyv[key] = FrameMerge(self.trackers), {n_: [] for n_ in self.trackers}, {}
+                for name, det in fixed.items():
+                    for f in range(f0, f0 + n):
+                        merges[key].put(name, f, det)
+                count[key] = f0 + n
+            for name, parts in out.items():
+                if name == ball_name:
+                    for key, f, (x, y, v) in parts:
+                        xyv[key][f] = (x, y, v)
+                        merges[key].put(name, f, Ball(frame=f, xy=(x, y), visibility=v))
+                else:
+                    for key, f0, objs in parts:
+                        for i, o in enumerate(objs):
+                            merges[key].put(name, f0 + i, o)
+            for key in ends:
+                if key not in merges:  # a stream of no frame
+                    merges[key], got[key], xyv[key] = FrameMerge(self.trackers), {n_: [] for n_ in self.trackers}, {}
+                if ball is not None:  # TrackNet gives no frame of a stream shorter than a window: no ball there
+                    for f in range(merges[key].next[ball_name], count.get(key, 0)):
+                        merges[key].put(ball_name, f, Ball(frame=f, xy=(0.0, 0.0), visibility=0))
+            ready = [(key, f, entry) for key in dict.fromkeys([r[0] for r in runs] + list(merges))
+                     for f, entry in merges[key].ready()]
+            for key, _, entry in ready:
+                for name, obj in entry.items():
+                    got[key][name].append(obj)
+            for key in ends:
+                res = got.pop(key)
+                if ball is not None:
+                    res[ball_name] = ball.balls(xyv.pop(key), count.pop(key, 0))  # InpaintNet over the trajectory
+                self.stream_results[key] = res
+                merges.pop(key)
+                mux.medians.pop(key, None)
+            return ready
+
+        pieces = mux.pieces()
+        steps = iter(())
+        if model:
+            for t in model.values():
+                t.to(t.DEVICE)
+            chunks = frames.chunks(pieces, B)
+            first = next(chunks, None)
+            if mux.hw is not None:  # a frame reached the pass
+                fp = StreamsPass(model, mux.hw, B, max_open, mux.metas, lambda key: mux.medians[key], self.video_info)
+                steps = (r for r in fp.run(itertools.chain([first], chunks)) if r is not None)
+            else:
+                steps = ((mux.metas.popleft(), {}) for _ in itertools.chain([first], chunks) if _ is not None)
+        else:
+            def direct():
+                for _ in pieces:
+                    while mux.metas:
+                        yield mux.metas.popleft(), {}
+                while mux.metas:
+                    yield mux.metas.popleft(), {}
+
+            steps = direct()
+        with self._clip_state():
+            for meta, out in steps:
+                yield from step(meta, out)
+        for t in model.values():
+            t.to("cpu")
+
     # ---- drawing pass (runner.py:91-173) -----------------------------------------------------------------------
     def _as_clip(self, frame_source) -> tuple[list, list, list]:
         """The run's video as the one clip of a drawing pass: ([frame source], [video_info], [results]), the clip as
@@ -570,8 +893,7 @@ class TrackingRunner:
         """Each clip restarts the trackers' order-dependent host stages (`video_info_post_init`: PlayerTracker gets a
         fresh ByteTrack); their `video_info` and ByteTrack are put back on exit, so a later run() finds them as they
         were."""
-        saved = {n: {k: t.__dict__[k] for k in ("video_info", "byte_track") if k in t.__dict__}
-                 for n, t in self.trackers.items()}
+        saved = {n: _host_state(t) for n, t in self.trackers.items()}
         try:
             yield
         finally:
