@@ -154,9 +154,29 @@ typedef struct pb_op_info {
   int N, H, W, C, c_off, c, out_C, out_coff;
   const float* weight;
   const float* bias;
+  int tw_log2, th_log2;     /* per-tap kernel: pixel tile TW = 2^tw_log2 x TH = 2^th_log2 x TN = 128 / (TW TH)   */
 } pb_op_info;
 /* Fills *out for op i; returns non-zero if i is out of range. */
 int pb_program_op_info(const pb_program* p, int i, pb_op_info* out);
+
+/* The tunable part of a conv plan: what a layer can change without changing the kernel the router picks for it or
+ * any output's accumulation order (channel block, tap, k-step).  Both kernels: the N tile BN and the persistent grid.
+ * Halo kernel: S, G, b_resident, a_stages, b_stages, tma_store; the rest must equal what pb_op_info reports.
+ * Per-tap kernel: the pixel tile (tw_log2, th_log2) and the ring depth `stages`; S = G = 1 and the halo fields 0.   */
+typedef struct pb_conv_plan {
+  int S, G, b_resident, a_stages, b_stages, tma_store;
+  int BN;
+  int tw_log2, th_log2, stages;
+  int grid;
+} pb_conv_plan;
+/* Every legal plan for descriptor d under the kernel the router picks for it: an instantiation exists, the rings and
+ * the staging tile fit the shared-memory budget, and pb_program_set_conv_plan accepts it.  Grids listed: all SMs and
+ * the fewest CTAs that take the same number of tile waves (any grid from 1 to that is legal too).  Writes up to
+ * `cap` plans to out (may be NULL when cap = 0) and returns how many there are, or -1 on error.                   */
+int pb_conv_list_plans(const pb_conv_desc* d, pb_conv_plan* out, int cap);
+/* Rebuild conv op i of p with `plan` (NULL: the router's default plan).  Non-zero, with op i left as it was, if the
+ * plan is not legal for the op's descriptor.                                                                      */
+int pb_program_set_conv_plan(pb_program* p, int i, const pb_conv_plan* plan);
 int pb_program_run(pb_program* p, void* stream);
 /* Run ops [first, last) only (per-layer timing / debugging). */
 int pb_program_run_range(pb_program* p, int first, int last, void* stream);

@@ -50,7 +50,25 @@ class OpInfo(C.Structure):
         ("N", C.c_int), ("H", C.c_int), ("W", C.c_int), ("C", C.c_int),
         ("c_off", C.c_int), ("c", C.c_int), ("out_C", C.c_int), ("out_coff", C.c_int),
         ("weight", C.c_void_p), ("bias", C.c_void_p),
+        ("tw_log2", C.c_int), ("th_log2", C.c_int),
     ]
+
+
+class ConvPlan(C.Structure):
+    """pb_conv_plan: the tunable fields of a conv plan (pb_conv_list_plans, pb_program_set_conv_plan)."""
+    _fields_ = [
+        ("S", C.c_int), ("G", C.c_int), ("b_resident", C.c_int), ("a_stages", C.c_int), ("b_stages", C.c_int),
+        ("tma_store", C.c_int),
+        ("BN", C.c_int),
+        ("tw_log2", C.c_int), ("th_log2", C.c_int), ("stages", C.c_int),
+        ("grid", C.c_int),
+    ]
+
+    def key(self) -> tuple:
+        return tuple(getattr(self, f) for f, _ in self._fields_)
+
+    def __repr__(self) -> str:
+        return "ConvPlan(" + ", ".join(f"{f}={getattr(self, f)}" for f, _ in self._fields_) + ")"
 
 
 class YoloLevel(C.Structure):
@@ -83,6 +101,8 @@ SIGNATURES = {
     "pb_program_op_info": (_i, [_p, _i, C.POINTER(OpInfo)]),
     "pb_program_run": (_i, [_p, _p]),
     "pb_program_run_range": (_i, [_p, _i, _i, _p]),
+    "pb_conv_list_plans": (_i, [C.POINTER(ConvDesc), C.POINTER(ConvPlan), _i]),
+    "pb_program_set_conv_plan": (_i, [_p, _i, C.POINTER(ConvPlan)]),
     "pb_letterbox_u8_f16": (_i, [_p, _i, _i, _i, _p, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p, _i, _i, _i, _i, _p]),
     "pb_pil_resize_u8": (_i, [_p, _i, _i, _i, _p, _p, _i, _i, _p, _p, _i, _p, _p, _i, _i, _p, _i, _p]),
     "pb_u8_to_f16_nhwc16": (_i, [_p, _i, _i, _i, _p, _i, _i, _i, _i, _p]),

@@ -159,6 +159,27 @@ int pb_program_add_pointwise_head(pb_program* p, const void* in, int N, int H, i
   return 0;
 }
 
+int pb_conv_list_plans(const pb_conv_desc* d, pb_conv_plan* out, int cap) {
+  if (!d || cap < 0 || (cap > 0 && !out)) {
+    set_error("conv_list_plans: bad argument");
+    return -1;
+  }
+  return conv_list_plans(d, out, cap);
+}
+
+int pb_program_set_conv_plan(pb_program* p, int i, const pb_conv_plan* plan) {
+  PB_CHECK(p != nullptr, "program_set_conv_plan: null");
+  PB_CHECK(i >= 0 && i < (int)p->ops.size() && p->ops[i].kind == OpKind::Conv,
+           "program_set_conv_plan: op %d is not a conv", i);
+  std::unique_ptr<ConvPlan> np(new ConvPlan());
+  const pb_conv_desc d = p->ops[i].conv->desc;
+  if (conv_plan_build(&d, np.get(), plan)) return 1;
+  PB_CHECK(np->variant == p->ops[i].conv->variant, "program_set_conv_plan: the plan changes op %d's kernel", i);
+  np->pdl = p->ops[i].conv->pdl;
+  p->ops[i].conv = std::move(np);
+  return 0;
+}
+
 int pb_program_num_ops(const pb_program* p) { return p ? (int)p->ops.size() : 0; }
 
 int pb_program_op_kernel(const pb_program* p, int i) {
@@ -207,6 +228,8 @@ int pb_program_op_info(const pb_program* p, int i, pb_op_info* out) {
       out->S = 1;
       out->G = 1;
       out->a_stages = out->b_stages = kp.stages;
+      out->tw_log2 = kp.tw_log2;
+      out->th_log2 = kp.th_log2;
     }
     out->grid = pl.grid;
     out->total_tiles = kp.total_tiles;

@@ -28,35 +28,53 @@ namespace pb {
 // shared memory for the rings and the staging tile (the tail and the alignment slack come on top, <= 227 KB)
 constexpr size_t kHaloSmemBudget = 196 * 1024;
 
-// TMA-store epilogue (conv_halo_kernel.cuh::halo_epilogue_tma) for an fp16 output without residual whose N tile is
-// stored whole: the staging tile (S * BN * 256 bytes) joins the rings inside the budget -- the weight ring down to four,
-// then the halo ring down to two, then the weight ring down to three stages; S and G stay as chosen.  Layers where it
-// does not fit, or does not apply, keep the per-lane store epilogue.  PADEL_B200_CONV_TMA_STORE=0 disables it (A/B).
-static int halo_plan_store(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode) {
-  const size_t budget = kHaloSmemBudget;
+static bool halo_store_enabled() {
   static const int enabled = [] {
     const char* e = getenv("PADEL_B200_CONV_TMA_STORE");
     return e ? atoi(e) : 1;
   }();
+  return enabled != 0;
+}
+
+// Whether the TMA-store epilogue can serve the layer, its N tiles covering `ntiles_bn` channels.
+static bool halo_store_applies(const pb_conv_desc* d, const ConvPlan* plan, int ntiles_bn) {
+  const bool f16 = d->out_mode == PB_OUT_F16_NHWC || d->out_mode == PB_OUT_F16_NHWC_UP2;
+  return plan->kp.dbg_flags == 0 && !d->res && d->head_n == 0 && f16 && plan->epi != PB_EPI_SILU_RES &&
+         d->cout_store == ntiles_bn && ((d->out_C | d->out_coff) & 7) == 0;
+}
+
+// TMA-store epilogue (conv_halo_kernel.cuh::halo_epilogue_tma) for an fp16 output without residual whose N tile is
+// stored whole: the staging tile (S * BN * 256 bytes) joins the rings inside the budget -- the weight ring down to four,
+// then the halo ring down to two, then the weight ring down to three stages; S and G stay as chosen.  Layers where it
+// does not fit, or does not apply, keep the per-lane store epilogue.  PADEL_B200_CONV_TMA_STORE=0 disables it (A/B).
+// A forced plan (fp) takes the epilogue it names with the rings it names; halo_finish_config checks that they fit.
+static int halo_plan_store(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode, const pb_conv_plan* fp) {
+  const size_t budget = kHaloSmemBudget;
   ConvKParams& kp = plan->kp;
   kp.st_bytes = 0;
   kp.st_maps = 0;
   kp.st_pool = 0;
-  const bool f16 = d->out_mode == PB_OUT_F16_NHWC || d->out_mode == PB_OUT_F16_NHWC_UP2;
-  if (!enabled || kp.dbg_flags != 0 || d->res || d->head_n != 0 || !f16 || plan->epi == PB_EPI_SILU_RES ||
-      d->cout_store != kp.n_ntiles * kp.BN || ((d->out_C | d->out_coff) & 7) != 0)
-    return 0;
-  // Deep-K streamed layers (more than two channel blocks) are mainloop-bound and need their third halo stage and
-  // deep weight ring more than an asynchronous epilogue (H100: up_block_2.conv_1 of TrackNet ran 5 % slower with it).
-  if (!kp.b_resident && kp.kblocks > 2) return 0;
+  const bool applies = halo_store_applies(d, plan, kp.n_ntiles * kp.BN);
   const uint32_t st = (uint32_t)kp.hs_S * (uint32_t)kp.BN * 256u;
   int as = kp.a_stages, bs = kp.b_stages;
-  auto total = [&] { return (size_t)as * kp.a_bytes + (size_t)bs * kp.b_bytes + st; };
-  while (total() > budget) {
-    if (!kp.b_resident && bs > 4) --bs;
-    else if (as > 2) --as;
-    else if (!kp.b_resident && bs > 3) --bs;
-    else return 0;
+  if (fp) {
+    if (!fp->tma_store) return 0;
+    PB_CHECK(applies, "conv(halo): the TMA-store epilogue does not apply to this layer");
+  } else {
+    if (!halo_store_enabled() || !applies) return 0;
+    // Streamed layers of one N tile and more than four channel blocks are mainloop-bound and need their deep weight
+    // ring more than an asynchronous epilogue: TrackNet's up_block_2.conv_1 (six blocks) ran 6 % faster with seven
+    // weight stages and per-lane stores than with the three the staging tile leaves.  With up to four blocks, or in
+    // N tiles, the TMA store wins: 7-18 % on TrackNet's N-tiled 256 / 512-channel layers and 11-14 % on up_block_3.conv_1
+    // (three blocks), at batch 32 and 8 (plan sweep, H100 80GB HBM3, 700 W; DESIGN 3.4).
+    if (!kp.b_resident && kp.kblocks > 4 && kp.n_ntiles == 1) return 0;
+    auto total = [&] { return (size_t)as * kp.a_bytes + (size_t)bs * kp.b_bytes + st; };
+    while (total() > budget) {
+      if (!kp.b_resident && bs > 4) --bs;
+      else if (as > 2) --as;
+      else if (!kp.b_resident && bs > 3) --bs;
+      else return 0;
+    }
   }
   // one map per destination of the staging box (channels, 8S columns, 8 rows, image); base = channel 0 of the slice,
   // which spans the N tiles' cout_store channels
@@ -97,20 +115,51 @@ static int halo_plan_store(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn 
   return 0;
 }
 
-// Launch configuration shared by the halo set-ups: one persistent CTA per SM.
-static void halo_finish_config(ConvPlan* plan) {
+static HaloKernelFn halo_kernel_pick(const ConvPlan* plan);
+
+// Launch configuration shared by the halo set-ups: one persistent CTA per SM, or the grid a forced plan names.  A
+// forced plan's rings are checked here against what the kernel and the shared-memory budget allow.
+static int halo_finish_config(ConvPlan* plan, const pb_conv_plan* fp) {
   const ConvKParams& kp = plan->kp;
-  plan->smem_bytes = (size_t)kp.a_stages * kp.a_bytes + (size_t)kp.b_stages * kp.b_bytes + kp.st_bytes +
-                     sizeof(HaloSmemTail) + 1024;
+  const size_t rings = (size_t)kp.a_stages * kp.a_bytes + (size_t)kp.b_stages * kp.b_bytes + kp.st_bytes;
+  plan->smem_bytes = rings + sizeof(HaloSmemTail) + 1024;
   plan->threads = kConvThreads;
-  plan->grid = kp.total_tiles < num_sms() ? kp.total_tiles : num_sms();
+  const int full = kp.total_tiles < num_sms() ? kp.total_tiles : num_sms();
+  plan->grid = full;
+  if (fp) {
+    PB_CHECK(rings <= kHaloSmemBudget, "conv(halo): plan needs %zu bytes of rings, budget %zu", rings,
+             kHaloSmemBudget);
+    PB_CHECK(kp.a_stages >= 2 && kp.a_stages <= kHaloMaxA, "conv(halo): a_stages %d outside 2..%d", kp.a_stages,
+             kHaloMaxA);
+    // a resident bank has one slot per (channel block, tap group); a streamed ring keeps one group in flight
+    const int bank = kp.kblocks * (kp.hs_ntaps / kp.hs_G);
+    PB_CHECK(kp.b_resident ? kp.b_stages == bank : kp.b_stages >= 2 && kp.b_stages <= kHaloMaxB,
+             "conv(halo): b_stages %d not legal (resident %d, bank %d)", kp.b_stages, kp.b_resident, bank);
+    PB_CHECK(halo_kernel_pick(plan) != nullptr, "conv(halo): no kernel instantiation for S=%d, k-steps=%d, N=%d",
+             kp.hs_S, kp.KB / 16, kp.BN);
+    if (fp->grid > 0) {
+      PB_CHECK(fp->grid <= full, "conv(halo): grid %d > %d", fp->grid, full);
+      plan->grid = fp->grid;
+    }
+  }
+  return 0;
 }
+
+// The fields a forced plan cannot change in a set-up whose S is its only tiling choice must equal the set-up's own.
+static int halo_fixed_fields(const ConvKParams& kp, const pb_conv_plan* fp) {
+  PB_CHECK(fp->G == kp.hs_G && fp->b_resident == kp.b_resident && fp->b_stages == kp.b_stages && fp->BN == kp.BN,
+           "conv(halo): G %d, resident %d, b_stages %d, BN %d are fixed at %d, %d, %d, %d for this layer", fp->G,
+           fp->b_resident, fp->b_stages, fp->BN, kp.hs_G, kp.b_resident, kp.b_stages, kp.BN);
+  return 0;
+}
+
+static bool halo_s_ok(int S, int BN) { return (S == 1 || S == 2 || S == 4) && S * ((BN + 31) / 32 * 32) <= 2 * kConvAccRegs; }
 
 // Stem (PB_IN_STEM4): 3x3 stride-2 conv over the padded 4-channel input. One TMA box of overlapping 16-element rows
 // (4 pixels x 4 channels, consecutive rows 2 pixels apart) holds, for a tile of 16 x 8S outputs, the three filter
 // rows r = 0..2 as [oh][r][ow] rows of 32 bytes; filter row r of sub-tile j starts at row (r*8S + 8j), 8-row groups
 // (consecutive oh) are 3*8S rows apart.  K = 16 per filter row (12 real), 3 wgmmas per sub-tile.
-int conv_stem_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode) {
+int conv_stem_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode, const pb_conv_plan* fp) {
   PB_CHECK(d->ksize == 3 && d->stride == 2 && d->C == 4 && d->cin == 16 && d->c_in_off == 0,
            "conv(stem): needs ksize 3, stride 2, C = 4, cin = 16");
   PB_CHECK(d->cout_pad <= 128, "conv(stem): cout_pad %d > 128", d->cout_pad);
@@ -119,6 +168,10 @@ int conv_stem_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode)
   const int acc_cols = (BN + 31) / 32 * 32;
   int S = 4;
   while (S > 1 && S * acc_cols > 2 * kConvAccRegs) S >>= 1;  // accumulators of S sub-tiles fit the registers
+  if (fp) {
+    PB_CHECK(halo_s_ok(fp->S, BN), "conv(stem): S %d not legal for N %d", fp->S, BN);
+    S = fp->S;
+  }
   kp.KB = 16;
   kp.kblocks = 1;
   kp.taps = 3;
@@ -159,12 +212,15 @@ int conv_stem_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode)
   kp.a_stages = 4;
   kp.b_stages = 1;  // the three filter rows are one small box: resident
   kp.b_resident = 1;
+  if (fp) {
+    if (halo_fixed_fields(kp, fp) != 0) return 1;
+    kp.a_stages = fp->a_stages;
+  }
   kp.tiles_w = (kp.Wo + 8 * S - 1) / (8 * S);
   kp.tiles_h = (kp.Ho + 15) / 16;
   kp.tiles_n = kp.N;
   kp.total_tiles = kp.tiles_w * kp.tiles_h * kp.tiles_n;
-  if (halo_plan_store(d, plan, encode) != 0) return 1;
-  halo_finish_config(plan);
+  if (halo_plan_store(d, plan, encode, fp) != 0 || halo_finish_config(plan, fp) != 0) return 1;
   plan->variant = 1;
   {
     // overlapping-row view of the padded (N, H+2, W+2, 4) tensor: element (k, ow, r, oh, n) =
@@ -209,12 +265,12 @@ int conv_stem_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode)
 // 64-channel layers trail; BN stays at 128.  Without `force` such a layer is taken only when the 16 x 8S tiles compute
 // at most 1.15x its output pixels (after the rows a warpgroup skips below the image): the per-tap kernel's flattened
 // 128-pixel tiles waste nothing at the edges.  `force`: wherever the kernel can run the layer.
-int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode, bool force) {
+int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode, bool force, const pb_conv_plan* fp) {
   if (d->ksize != 3 || d->stride != 1) return -1;
   const bool ntiled = d->cout_pad > 192 && d->cout_pad % kHaloNTileBN == 0 && d->head_n == 0;
   if (!ntiled && d->cout_pad > (force ? 256 : 192)) return -1;
   ConvKParams& kp = plan->kp;  // common fields (epilogue, KB, kblocks, ...) already filled by the caller
-  const int BN = ntiled ? kHaloNTileBN : d->cout_pad;
+  int BN = ntiled ? kHaloNTileBN : d->cout_pad;
   const uint32_t row_bytes = (uint32_t)kp.KB * 2u;
   const int acc_cols = (BN + 31) / 32 * 32;
   const size_t budget = kHaloSmemBudget;
@@ -231,7 +287,11 @@ int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode,
     const char* er = getenv("PADEL_B200_CONV_BRES");
     resident = (!er || atoi(er) != 0) && !ntiled && kp.kblocks <= kHaloMaxB && res_total <= 120 * 1024;
   }
+  // The staging tile of the TMA-store epilogue at sub-tile count S (0 when that epilogue cannot serve the layer)
+  const bool store = halo_store_enabled() && halo_store_applies(d, plan, d->cout_pad);
+  auto staging = [&](int S) { return store ? (size_t)S * BN * 256u : 0; };
   int bestS = 0, best_cols = 0, G = 1;
+  bool best_st = false;
   for (int pass = resident ? 0 : 1; pass < 2 && bestS == 0; ++pass) {
     resident = resident && pass == 0;
     for (int S = 4; S >= 1; S >>= 1) {
@@ -253,21 +313,49 @@ int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode,
       }
       if (!g_fit) continue;
       const int cols = (d->W + 8 * S - 1) / (8 * S) * 8 * S;  // padded width actually computed
-      // resident: prefer the largest S that fits (less halo overlap); streaming: the least padding
-      if (bestS == 0 || (!resident && cols < best_cols)) {
+      // resident: the largest S that fits beside the TMA-store staging tile, else the largest that fits (a smaller
+      // S with TMA stores beat a larger one without: 13-15 % on the 64 -> 96 layers of the pose and court programs).
+      // streaming: the least padding, S = 2 on a tie with S = 4 -- at S = 4 the staging tile does not fit beside two
+      // halos, and TrackNet's up_block_3.conv_1 ran 11-14 % faster at S = 2 with TMA stores.
+      const bool st_fit = resident && store && (size_t)2 * a_alloc + res_total + staging(S) <= budget;
+      if (bestS == 0 || (resident && st_fit && !best_st) ||
+          (!resident && (cols < best_cols || (cols == best_cols && S == 2)))) {
         bestS = S;
         best_cols = cols;
         G = g_fit;
+        best_st = st_fit;
       }
     }
   }
-  const uint32_t b_alloc = ((uint32_t)G * tap_bytes + 1023u) & ~1023u;
   if (bestS == 0) return -1;
-  const int S = bestS, P = 8 * S + 2;
+  int S = bestS;
   if (ntiled && !force) {
     const long computed = (long)best_cols * ((kp.Ho + 7) / 8 * 8);
     if (20 * computed > 23 * (long)kp.Wo * kp.Ho) return -1;
   }
+  if (!resident && !ntiled && d->out_mode == PB_OUT_F16_NHWC_UP2 && store) {
+    // x2 upsampled output through the staging tile: S = 1 halves the tile and leaves the weight ring seven stages
+    // instead of three (TrackNet's up_block_2.conv_2: 15-18 % faster at batch 32 and 8)
+    S = 1;
+    G = 1;
+  }
+  if (fp) {
+    // N split: the whole cout_pad in one tile, or N tiles of kHaloNTileBN (the only instantiations that carry the N
+    // tile index); a resident bank holds all nine taps of one N tile
+    const bool bn_ok = fp->BN == d->cout_pad ? d->cout_pad <= 256
+                                             : fp->BN == kHaloNTileBN && d->cout_pad % kHaloNTileBN == 0 && d->head_n == 0;
+    PB_CHECK(bn_ok, "conv(halo): BN %d not legal for cout_pad %d", fp->BN, d->cout_pad);
+    PB_CHECK(halo_s_ok(fp->S, fp->BN), "conv(halo): S %d not legal for N %d", fp->S, fp->BN);
+    PB_CHECK(fp->G == 1 || fp->G == 3 || fp->G == 9, "conv(halo): G %d not in {1, 3, 9}", fp->G);
+    PB_CHECK(!fp->b_resident || (fp->G == 9 && fp->BN == d->cout_pad && kp.kblocks <= kHaloMaxB),
+             "conv(halo): a resident bank needs G = 9, one N tile and at most %d channel blocks", kHaloMaxB);
+    BN = fp->BN;
+    S = fp->S;
+    G = fp->G;
+    resident = fp->b_resident != 0;
+  }
+  const int P = 8 * S + 2;
+  const uint32_t b_alloc = ((uint32_t)G * (uint32_t)BN * row_bytes + 1023u) & ~1023u;
   kp.b_resident = resident ? 1 : 0;
   kp.hs_S = S;
   kp.hs_P = P;
@@ -286,7 +374,7 @@ int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode,
   kp.halo_bytes = 18u * (uint32_t)P * row_bytes;
   kp.hs_a_row_bytes = row_bytes;
   kp.a_bytes = (kp.halo_bytes + 1023u) & ~1023u;
-  kp.b_tx_bytes = (uint32_t)G * tap_bytes;
+  kp.b_tx_bytes = (uint32_t)G * (uint32_t)BN * row_bytes;
   kp.b_bytes = b_alloc;
   kp.a_stages = 2;
   if (resident) {
@@ -297,23 +385,24 @@ int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode,
     if (as > 2 * kp.kblocks + 1) as = 2 * kp.kblocks + 1;
     kp.a_stages = as < 2 ? 2 : as;
   } else {
-    size_t rest = budget - (size_t)2 * kp.a_bytes;
-    if (kp.kblocks > 2 && rest > (size_t)kp.a_bytes + 4 * (size_t)b_alloc) {  // a third halo buffer when K is deep
-      kp.a_stages = 3;
-      rest -= kp.a_bytes;
-    }
+    // two halo buffers, the rest to weight stages (a third halo buffer in their place ran TrackNet's up_block_2.conv_1
+    // 3-6 % slower)
+    const size_t rest = budget - (size_t)2 * kp.a_bytes;
     int bs = (int)(rest / b_alloc);
     if (bs > kHaloMaxB) bs = kHaloMaxB;
     if (bs > 9 * kp.kblocks / G * 2) bs = 9 * kp.kblocks / G * 2;
     if (bs < 2) bs = 2;
     kp.b_stages = bs;
   }
+  if (fp) {
+    kp.a_stages = fp->a_stages;
+    kp.b_stages = fp->b_stages;
+  }
   kp.tiles_w = (kp.Wo + 8 * S - 1) / (8 * S);
   kp.tiles_h = (kp.Ho + 15) / 16;
   kp.tiles_n = kp.N;
   kp.total_tiles = kp.tiles_w * kp.tiles_h * kp.tiles_n * kp.n_ntiles;
-  if (halo_plan_store(d, plan, encode) != 0) return 1;
-  halo_finish_config(plan);
+  if (halo_plan_store(d, plan, encode, fp) != 0 || halo_finish_config(plan, fp) != 0) return 1;
   plan->variant = 1;
 
   const CUtensorMapSwizzle swz = kp.KB == 64   ? CU_TENSOR_MAP_SWIZZLE_128B
@@ -350,7 +439,7 @@ int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode,
 // often.  That pays off for the narrow layers of the pose program (cin 32 -> 32 @320^2); wider layers stay on the
 // per-tap kernel, whose flattened 128-pixel tiles waste nothing at the image edges and whose K loop is deeper.  Default rule therefore: cin <= 32; PADEL_B200_CONV_HALO1=0 disables it, =2
 // takes every 1x1 layer whose bank fits next to two activation buffers.
-int conv_halo_1x1_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode) {
+int conv_halo_1x1_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode, const pb_conv_plan* fp) {
   static const int enabled = [] {
     const char* e = getenv("PADEL_B200_CONV_HALO1");
     return e ? atoi(e) : 1;
@@ -378,6 +467,10 @@ int conv_halo_1x1_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn enc
     break;
   }
   if (S == 0) return -1;
+  if (fp) {
+    PB_CHECK(halo_s_ok(fp->S, BN), "conv(halo 1x1): S %d not legal for N %d", fp->S, BN);
+    S = fp->S;
+  }
   const int P = 8 * S;
   kp.b_resident = 1;
   kp.hs_S = S;
@@ -403,12 +496,15 @@ int conv_halo_1x1_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn enc
     if (as > 2 * kp.kblocks + 1) as = 2 * kp.kblocks + 1;
     kp.a_stages = as < 2 ? 2 : as;
   }
+  if (fp) {
+    if (halo_fixed_fields(kp, fp) != 0) return 1;
+    kp.a_stages = fp->a_stages;
+  }
   kp.tiles_w = (kp.Wo + 8 * S - 1) / (8 * S);
   kp.tiles_h = (kp.Ho + 15) / 16;
   kp.tiles_n = kp.N;
   kp.total_tiles = kp.tiles_w * kp.tiles_h * kp.tiles_n;
-  if (halo_plan_store(d, plan, encode) != 0) return 1;
-  halo_finish_config(plan);
+  if (halo_plan_store(d, plan, encode, fp) != 0 || halo_finish_config(plan, fp) != 0) return 1;
   plan->variant = 1;
   const CUtensorMapSwizzle swz = kp.KB == 64   ? CU_TENSOR_MAP_SWIZZLE_128B
                                  : kp.KB == 32 ? CU_TENSOR_MAP_SWIZZLE_64B
@@ -447,7 +543,7 @@ int conv_halo_1x1_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn enc
 // i.e. again only a descriptor start offset (row offset * 4C + half * 2C bytes) with SBO = 2P rows, and K = C per tap
 // (the 32-byte k-step advance inside the swizzle row is the usual one).  Versus nine per-tap boxes of 2C-byte rows
 // this issues one TMA per tile with rows twice as long (TMA delivery of 32-byte rows is what bounds the per-tap path).
-int conv_halo_s2_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode) {
+int conv_halo_s2_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode, const pb_conv_plan* fp) {
   if (d->ksize != 3 || d->stride != 2 || d->cout_pad > 256 || d->c_in_off != 0 || d->C != d->cin ||
       (d->cin != 16 && d->cin != 32))
     return -1;
@@ -469,6 +565,10 @@ int conv_halo_s2_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn enco
     }
   }
   if (S == 0) return -1;
+  if (fp) {
+    PB_CHECK(halo_s_ok(fp->S, BN), "conv(halo s2): S %d not legal for N %d", fp->S, BN);
+    S = fp->S;
+  }
   const int P = 8 * S + 1;
   kp.KB = d->cin;
   kp.kblocks = 1;
@@ -496,12 +596,15 @@ int conv_halo_s2_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn enco
   kp.a_stages = 2;
   kp.b_stages = 1;  // all nine taps are one box: resident
   kp.b_resident = 1;
+  if (fp) {
+    if (halo_fixed_fields(kp, fp) != 0) return 1;
+    kp.a_stages = fp->a_stages;
+  }
   kp.tiles_w = (kp.Wo + 8 * S - 1) / (8 * S);
   kp.tiles_h = (kp.Ho + 15) / 16;
   kp.tiles_n = kp.N;
   kp.total_tiles = kp.tiles_w * kp.tiles_h * kp.tiles_n;
-  if (halo_plan_store(d, plan, encode) != 0) return 1;
-  halo_finish_config(plan);
+  if (halo_plan_store(d, plan, encode, fp) != 0 || halo_finish_config(plan, fp) != 0) return 1;
   plan->variant = 1;
   {
     const cuuint64_t C = (cuuint64_t)d->C, W = (cuuint64_t)d->W, H = (cuuint64_t)d->H;

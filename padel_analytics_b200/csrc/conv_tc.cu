@@ -15,6 +15,7 @@
 // (reference trackers/ball_tracker/models.py:5-17) with BN folded into weight/bias.
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <mutex>
 
 #include "internal.h"
@@ -227,7 +228,7 @@ int conv_epi_class(const pb_conv_desc* d, const ConvKParams& kp) {
   return d->act == PB_ACT_SILU ? PB_EPI_SILU : (d->act == PB_ACT_RELU ? PB_EPI_RELU : PB_EPI_GENERIC);
 }
 
-static int conv_plan_build_impl(const pb_conv_desc* d, ConvPlan* plan) {
+static int conv_plan_build_impl(const pb_conv_desc* d, ConvPlan* plan, const pb_conv_plan* fp) {
   PB_CHECK(d && plan, "conv: null argument");
   PB_CHECK(d->in_layout == PB_IN_NHWC || d->in_layout == PB_IN_STEM4, "conv: bad in_layout");
   const bool stem = d->in_layout == PB_IN_STEM4;
@@ -316,7 +317,7 @@ static int conv_plan_build_impl(const pb_conv_desc* d, ConvPlan* plan) {
   plan->variant = 0;
   plan->pdl = plan_pdl();
   plan->epi = conv_epi_class(d, kp);
-  if (stem) return conv_stem_setup(d, plan, encode);
+  if (stem) return conv_stem_setup(d, plan, encode, fp);
   {
     // halo variant: default on for cout <= 192 (the layers the per-tap kernel leaves L2/TMA-bound) and for the 3x3 / s1
     // layers conv_halo_setup runs in N tiles with little edge waste; PADEL_B200_CONV_HALO=0 disables it, =1 forces it
@@ -325,9 +326,9 @@ static int conv_plan_build_impl(const pb_conv_desc* d, ConvPlan* plan) {
     const int mode = e ? atoi(e) : 2;
     const bool s1_3x3 = d->ksize == 3 && d->stride == 1;
     if (mode == 1 || (mode == 2 && (d->cout_pad <= 192 || s1_3x3))) {
-      const int rc = d->ksize == 1    ? conv_halo_1x1_setup(d, plan, encode)
-                     : d->stride == 2 ? conv_halo_s2_setup(d, plan, encode)
-                                      : conv_halo_setup(d, plan, encode, mode == 1 || d->out2_mode == PB_OUT2_POOL2);
+      const int rc = d->ksize == 1    ? conv_halo_1x1_setup(d, plan, encode, fp)
+                     : d->stride == 2 ? conv_halo_s2_setup(d, plan, encode, fp)
+                                      : conv_halo_setup(d, plan, encode, mode == 1 || d->out2_mode == PB_OUT2_POOL2, fp);
       if (rc >= 0) return rc;
     }
   }
@@ -339,6 +340,14 @@ static int conv_plan_build_impl(const pb_conv_desc* d, ConvPlan* plan) {
   kp.n_ntiles = nn;
   kp.BN = d->cout_pad / nn;
   PB_CHECK(kp.BN >= 16 && kp.BN <= 256, "conv: cannot tile cout_pad %d", d->cout_pad);
+  if (fp) {
+    PB_CHECK(fp->BN >= 16 && fp->BN <= 256 && fp->BN % 16 == 0 && d->cout_pad % fp->BN == 0,
+             "conv: BN %d does not tile cout_pad %d", fp->BN, d->cout_pad);
+    PB_CHECK(fp->S == 1 && fp->G == 1 && fp->b_resident == 0 && fp->tma_store == 0,
+             "conv: the per-tap kernel has no halo plan fields");
+    kp.BN = fp->BN;
+    kp.n_ntiles = d->cout_pad / fp->BN;
+  }
 
   // pixel tile shape (TN x TH x TW = 128): minimise the number of tiles, prefer wide tiles
   long best_cost = -1;
@@ -353,6 +362,12 @@ static int conv_plan_build_impl(const pb_conv_desc* d, ConvPlan* plan) {
         best_th = thl;
       }
     }
+  }
+  if (fp) {
+    PB_CHECK(fp->tw_log2 >= 2 && fp->tw_log2 <= 7 && fp->th_log2 >= 0 && fp->tw_log2 + fp->th_log2 <= 7,
+             "conv: pixel tile 2^%d x 2^%d not legal", fp->tw_log2, fp->th_log2);
+    best_tw = fp->tw_log2;
+    best_th = fp->th_log2;
   }
   kp.tw_log2 = best_tw;
   kp.th_log2 = best_th;
@@ -387,10 +402,19 @@ static int conv_plan_build_impl(const pb_conv_desc* d, ConvPlan* plan) {
   int stages = (int)(kConvStageBudget / stage_bytes);
   if (stages > kConvMaxStages) stages = kConvMaxStages;
   PB_CHECK(stages >= 2, "conv: stage too large (%u bytes)", stage_bytes);
+  if (fp) {
+    PB_CHECK(fp->stages >= 2 && fp->stages <= stages, "conv: %d stages of %u bytes do not fit (at most %d)", fp->stages,
+             stage_bytes, stages);
+    stages = fp->stages;
+  }
   kp.stages = stages;
   plan->smem_bytes = (size_t)stages * stage_bytes + sizeof(ConvSmemTail) + 1024;
   plan->threads = kConvThreads;
   plan->grid = kp.total_tiles < num_sms() ? kp.total_tiles : num_sms();
+  if (fp && fp->grid > 0) {
+    PB_CHECK(fp->grid <= plan->grid, "conv: grid %d > %d", fp->grid, plan->grid);
+    plan->grid = fp->grid;
+  }
   const CUtensorMapSwizzle swz = kp.KB == 64   ? CU_TENSOR_MAP_SWIZZLE_128B
                                  : kp.KB == 32 ? CU_TENSOR_MAP_SWIZZLE_64B
                                                : CU_TENSOR_MAP_SWIZZLE_32B;
@@ -427,14 +451,82 @@ static int conv_plan_build_impl(const pb_conv_desc* d, ConvPlan* plan) {
   return 0;
 }
 
-int conv_plan_build(const pb_conv_desc* d, ConvPlan* plan) {
-  const int rc = conv_plan_build_impl(d, plan);
+int conv_plan_build(const pb_conv_desc* d, ConvPlan* plan, const pb_conv_plan* fp) {
+  const int rc = conv_plan_build_impl(d, plan, fp);
   if (rc == 0) {
     plan->kp.fd_w = make_fastdiv(plan->kp.tiles_w);
     plan->kp.fd_h = make_fastdiv(plan->kp.tiles_h);
     plan->kp.fd_nt = make_fastdiv(plan->kp.n_ntiles);
   }
   return rc;
+}
+
+// The tunable fields of a built plan (pb_conv_plan); the fields the plan's kernel does not have are 0.
+static pb_conv_plan conv_plan_fields(const ConvPlan& pl) {
+  const ConvKParams& kp = pl.kp;
+  pb_conv_plan f;
+  memset(&f, 0, sizeof(f));
+  f.BN = kp.BN;
+  f.grid = pl.grid;
+  if (pl.variant == 1) {
+    f.S = kp.hs_S;
+    f.G = kp.hs_G;
+    f.b_resident = kp.b_resident;
+    f.a_stages = kp.a_stages;
+    f.b_stages = kp.b_stages;
+    f.tma_store = kp.st_bytes != 0;
+  } else {
+    f.S = f.G = 1;
+    f.tw_log2 = kp.tw_log2;
+    f.th_log2 = kp.th_log2;
+    f.stages = kp.stages;
+  }
+  return f;
+}
+
+// Every combination of the tunable fields, built one by one: the legal plans are those conv_plan_build accepts under
+// the default plan's kernel.  The grid takes two values per tiling: one CTA per SM, and the fewest CTAs that keep the
+// same number of tile waves.
+int conv_list_plans(const pb_conv_desc* d, pb_conv_plan* out, int cap) {
+  std::unique_ptr<ConvPlan> def(new ConvPlan()), tmp(new ConvPlan());
+  if (conv_plan_build(d, def.get())) return -1;
+  const int variant = def->variant;
+  int count = 0;
+  auto try_plan = [&](pb_conv_plan c) {
+    for (int pass = 0; pass < 2; ++pass) {
+      c.grid = 0;
+      if (conv_plan_build(d, tmp.get(), &c) != 0 || tmp->variant != variant) return;
+      const int full = tmp->grid, tiles = tmp->kp.total_tiles, waves = (tiles + full - 1) / full;
+      c.grid = pass == 0 ? full : (tiles + waves - 1) / waves;
+      if (pass == 1 && c.grid == full) return;
+      if (count < cap) out[count] = c;
+      ++count;
+    }
+  };
+  pb_conv_plan c;
+  memset(&c, 0, sizeof(c));
+  if (variant == 1) {
+    for (int bn = 16; bn <= 256; bn += 16)
+      for (int S = 1; S <= 4; S *= 2)
+        for (int G : {1, 3, 9})
+          for (int res = 0; res <= 1; ++res)
+            for (int as = 2; as <= 4; ++as)
+              for (int bs = 1; bs <= kConvMaxStages; ++bs)
+                for (int tma = 0; tma <= 1; ++tma) {
+                  c.BN = bn, c.S = S, c.G = G, c.b_resident = res, c.a_stages = as, c.b_stages = bs, c.tma_store = tma;
+                  if (d->cout_pad % bn == 0) try_plan(c);
+                }
+  } else {
+    c.S = c.G = 1;
+    for (int bn = 16; bn <= 256; bn += 16)
+      for (int tw = 2; tw <= 7; ++tw)
+        for (int th = 0; tw + th <= 7; ++th)
+          for (int st = 2; st <= kConvMaxStages; ++st) {
+            c.BN = bn, c.tw_log2 = tw, c.th_log2 = th, c.stages = st;
+            if (d->cout_pad % bn == 0) try_plan(c);
+          }
+  }
+  return count;
 }
 
 int conv_plan_launch(const ConvPlan* plan, cudaStream_t stream) {

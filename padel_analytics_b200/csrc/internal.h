@@ -181,12 +181,18 @@ int conv_epi_class(const pb_conv_desc* d, const ConvKParams& kp);
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode, bool force);  // -1: not applicable
-int conv_stem_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode);
-int conv_halo_s2_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode);  // -1: not applicable
-int conv_halo_1x1_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode);  // -1: not applicable
+// The set-ups choose a plan by their rules, or take the tunable fields from `fp` (pb_conv_plan) when it is not null;
+// the choice of set-up (the routing) never depends on fp.
+int conv_halo_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode, bool force,
+                    const pb_conv_plan* fp);  // -1: not applicable
+int conv_stem_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode, const pb_conv_plan* fp);
+int conv_halo_s2_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode,
+                       const pb_conv_plan* fp);  // -1: not applicable
+int conv_halo_1x1_setup(const pb_conv_desc* d, ConvPlan* plan, EncodeTiledFn encode,
+                        const pb_conv_plan* fp);  // -1: not applicable
 int conv_halo_launch(const ConvPlan* plan, cudaStream_t stream);
-int conv_plan_build(const pb_conv_desc* d, ConvPlan* plan);
+int conv_plan_build(const pb_conv_desc* d, ConvPlan* plan, const pb_conv_plan* fp = nullptr);
+int conv_list_plans(const pb_conv_desc* d, pb_conv_plan* out, int cap);  // pb_conv_list_plans
 int conv_plan_launch(const ConvPlan* plan, cudaStream_t stream);
 int conv_reference_launch(const pb_conv_desc* d, cudaStream_t stream);
 

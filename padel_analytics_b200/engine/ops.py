@@ -201,11 +201,41 @@ class Program:
         L.check(L.lib().pb_program_op_info(self._h, i, C.byref(info)))
         return info
 
+    def conv_plan(self, i: int) -> L.ConvPlan:
+        """The tunable fields of conv op i's plan (as pb_conv_list_plans lists them)."""
+        return plan_of(self.op_info(i))
+
+    def conv_plans(self, i: int) -> list[L.ConvPlan]:
+        """Every legal plan for conv op i's descriptor under the kernel it runs (pb_conv_list_plans)."""
+        info = self.op_info(i)
+        n = L.lib().pb_conv_list_plans(C.byref(info.desc), None, 0)
+        L.check(int(n < 0))
+        plans = (L.ConvPlan * n)()
+        L.check(int(L.lib().pb_conv_list_plans(C.byref(info.desc), plans, n) != n))
+        return list(plans)
+
+    def set_conv_plan(self, i: int, plan: L.ConvPlan | None):
+        """Rebuild conv op i with `plan`, or with the default plan when None (pb_program_set_conv_plan)."""
+        L.check(L.lib().pb_program_set_conv_plan(self._h, i, C.byref(plan) if plan is not None else None))
+
     def run(self, first: int | None = None, last: int | None = None):
         if first is None:
             L.check(L.lib().pb_program_run(self._h, L.stream_ptr()))
         else:
             L.check(L.lib().pb_program_run_range(self._h, first, last, L.stream_ptr()))
+
+
+def plan_of(info: L.OpInfo) -> L.ConvPlan:
+    """The pb_conv_plan fields of the conv plan pb_op_info describes."""
+    p = L.ConvPlan()
+    p.BN, p.grid = info.BN, info.grid
+    if info.variant == L.CONV_PER_TAP:
+        p.S = p.G = 1
+        p.tw_log2, p.th_log2, p.stages = info.tw_log2, info.th_log2, info.a_stages
+    else:
+        p.S, p.G, p.b_resident = info.S, info.G, info.b_resident
+        p.a_stages, p.b_stages, p.tma_store = info.a_stages, info.b_stages, info.tma_store
+    return p
 
 
 def time_program_ops(prog: Program, repeats: int = 5):
